@@ -52,9 +52,16 @@ tests/cpp/tick_host_test: $(TICKHOST_DEP)
 	$(CXX) -std=c++17 -O1 -I$(CUDA_INC) -pthread -o $@ $(TICKHOST_SRC)
 tests/cpp/tick_host_test_san: $(TICKHOST_DEP)
 	$(SAN_CXX) -std=c++17 -O0 -fsanitize=address,undefined -fno-sanitize-recover=undefined -I$(CUDA_INC) -pthread -o $@ $(TICKHOST_SRC)
+# The same at the library's 16-bit offset width (it includes tick_host_test.cpp for the harness).
+TICKHOST16_SRC := tests/cpp/tick_host16_test.cpp oracle/raft_oracle.c
+TICKHOST16_DEP := $(TICKHOST16_SRC) $(TICKHOST_DEP)
+tests/cpp/tick_host16_test: $(TICKHOST16_DEP)
+	$(CXX) -std=c++17 -O1 -I$(CUDA_INC) -pthread -o $@ $(TICKHOST16_SRC)
+tests/cpp/tick_host16_test_san: $(TICKHOST16_DEP)
+	$(SAN_CXX) -std=c++17 -O0 -fsanitize=address,undefined -fno-sanitize-recover=undefined -I$(CUDA_INC) -pthread -o $@ $(TICKHOST16_SRC)
 
 clean:
 	rm -f $(LIB) $(HOSTLIB) $(CPPTEST) tests/cpp/raftpipe_test_asan tests/cpp/raftpipe_test_tsan build_ptxas.log \
-	  tests/cpp/tick_host_test tests/cpp/tick_host_test_san
+	  tests/cpp/tick_host_test tests/cpp/tick_host_test_san tests/cpp/tick_host16_test tests/cpp/tick_host16_test_san
 	$(MAKE) -C oracle clean
 .PHONY: all oracle clean san_cxx

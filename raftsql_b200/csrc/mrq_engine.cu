@@ -128,8 +128,8 @@ struct mrq_engine {
   uint64_t *peer_gather[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   bool ipc_attached = false;
   int quorum_variant = 1;  // 0 = quad (4 groups/thread, 2 x LDG.128 per column), 1 = TMA bulk (fastest on H100), 2 = LDG.128
-  // tick mode 4: compact state (32-bit offsets from a per-group base) + the byte inbox, four groups per thread
-  CompactView c{};
+  // tick mode 4: compact state (16-bit offsets from a per-group base) + the byte inbox, four groups per thread
+  CompactViewT<CompactOff> c{};
   bool compact_alloc = false;  // the compact columns exist
   bool compact_live = false;   // some groups may be compact-authoritative (wide columns stale for them)
   unsigned long long *slow_list64 = nullptr;
@@ -307,7 +307,7 @@ void fill_tick_args(mrq_engine *e, TickArgs &a) {
 int launch_tick4(mrq_engine *e, const uint32_t *slots, uint32_t n) {
   int r = ensure_compact(e);
   if (r) return r;
-  Tick4Args A{};
+  Tick4ArgsT<CompactOff> A{};
   fill_tick_args(e, A.t);
   A.c = e->c;
   A.base_index = e->pk_base_index;

@@ -147,7 +147,7 @@ __device__ __forceinline__ void st_state_u32(uint32_t *p, uint32_t v) {
 
 // ---- L2 residency policy --------------------------------------------------------------------------------
 // Every tick streams its inbox through L2 exactly once while the engine state is re-read every tick (the compact
-// state of tick mode 4 is ~47 MB at the headline shape, next to H100's 50 MB L2).  Left alone the stream evicts the
+// state of tick mode 4 is ~30 MB at the headline shape, next to H100's 50 MB L2).  Left alone the stream evicts the
 // state and each tick re-reads it from HBM.  With cache-hinted accesses (createpolicy + .L2::cache_hint; the
 // policy rides in the memory descriptor, no extra instructions) the inbox is marked evict-first and the state
 // evict-last, so state columns stay on-chip from one tick to the next and HBM mostly carries the inbox.
@@ -1147,7 +1147,7 @@ __global__ void __launch_bounds__(kTickThreads, (R <= 5 ? 6 : 5)) tick_general_k
 
 // ==== tick mode 4: the tick on COMPACT state + the byte inbox =====================================================
 // The wide layout moves 217 B per group-tick at R = 5 (DESIGN.md §4.1), most of it 64-bit indices whose upper halves
-// never change.  In mode 4 every index-like column of a group is a 32-bit OFFSET from one per-group u64 base
+// never change.  In mode 4 every index-like column of a group is a 16-bit OFFSET from one per-group u64 base
 // `ibase[g]` that only the general path ever reads:
 //     c.commit[g]        committed  - ibase
 //     c.match[j][g]      Progress.Match of the j-th REMOTE sender - ibase, j = 0..R-2 in ascending id order — the row order
@@ -1160,11 +1160,13 @@ __global__ void __launch_bounds__(kTickThreads, (R <= 5 ? 6 : 5)) tick_general_k
 //                         window base), CF_TERM_OK (base_term == term: window messages carry the group's term),
 //                         CF_GATE_OPEN (leader, term_start <= committed: the commit gate can no longer block)
 // term, term_start, last_term never change on the fast path: they stay wide and are never read by it.  With the byte
-// inbox (R-1 sender bytes + 1 proposal byte) the steady-state tick reads 8 (meta) + 1 + 4 + 4 + 4R + R = 42 B and
-// writes 8 + 4 (out) + 1 (commit advance) + 4 + 4 + 4(R-1) + 3 = 40 B per group at R = 5: 82 B instead of 217.
-// One thread owns FOUR adjacent groups: every column access is one 128-bit (u32 x 4) or two 128-bit (u64 x 4) loads or
-// stores, which also cuts the instruction count per group-tick to a quarter of the scalar kernels'.
-// Exactness: a group whose values do not fit (2^31 entries from its base), whose tick needs the role machinery, or
+// inbox (R-1 sender bytes + 1 proposal byte) the steady-state tick reads 8 (meta) + 1 + 2 + 2 + 2R + R = 28 B and
+// writes 8 + 4 (out) + 1 (commit advance) + 2 + 2 + 2(R-1) + 1.5 = 26.5 B per group at R = 5: 54.5 B instead of 217.
+// One thread owns FOUR adjacent groups: every column access is one 64-bit (u16 x 4), 128-bit (u32 x 4) or two 128-bit
+// (u64 x 4) loads or stores, which also cuts the instruction count per group-tick to a quarter of the scalar kernels'.
+// Sixteen bits hold ~43k ticks of log growth at the steady trace's 1.5 proposals per tick; a group that outgrows
+// them is re-based by the general path (compact_group picks a fresh base), exactly as a 32-bit one would be.
+// Exactness: a group whose values do not fit (compact_span entries from its base), whose tick needs the role machinery, or
 // whose frame holds anything but in-window acks / its leader's heartbeat is handed to the general path, which
 // materialises the wide columns, runs the unchanged general tick on them, and re-compacts.
 enum : uint32_t { CF_COMPACT = 1u, CF_TERM_OK = 2u, CF_GATE_OPEN = 4u };
@@ -1175,15 +1177,27 @@ static constexpr uint32_t kCompactSpan = 0x7FFFFFFFu;  // offsets stay below 2^3
 static uint32_t kCompactSpan = 0x7FFFFFFFu;  // (the host test lowers it to drive groups through the re-base path)
 #endif
 
-struct CompactView {
-  uint8_t *flag;     // [gs]
-  uint32_t *commit;  // [gs]
-  uint32_t *win;     // [gs]
-  uint32_t *gate;    // [gs]
-  uint32_t *iblo;    // [gs] low word of ibase (fused gather only)
-  uint32_t *match;   // [R][gs]
-  uint64_t *ibase;   // [gs]
+// The offset columns are `Off` wide in memory (the library: uint16_t; the host test also runs uint32_t); in registers
+// every offset is a uint32_t.  The span an offset may reach is kCompactSpan clamped to the width minus one, so that
+// the largest value of the type stays free for a gate that is closed for good (compact_group).
+typedef uint16_t CompactOff;
+template <typename Off>
+__device__ __forceinline__ uint32_t compact_span() {
+  const uint32_t w = (uint32_t)static_cast<Off>(~Off(0)) - 1u;
+  return kCompactSpan < w ? kCompactSpan : w;
+}
+
+template <typename Off = uint32_t>
+struct CompactViewT {
+  uint8_t *flag;    // [gs]
+  Off *commit;      // [gs]
+  Off *win;         // [gs]
+  Off *gate;        // [gs]
+  uint32_t *iblo;   // [gs] low word of ibase (fused gather only)
+  Off *match;       // [R][gs]
+  uint64_t *ibase;  // [gs]
 };
+using CompactView = CompactViewT<>;
 
 template <int R>
 struct CGroup {  // one group's compact state, in registers
@@ -1202,7 +1216,7 @@ __host__ __device__ __forceinline__ uint32_t crow_sender(uint32_t j, uint32_t se
 
 // The HOT case of a tick, straight-line: a settled leader (no strict mode, lastTerm == Term) whose frame holds nothing
 // but in-window acks of its own term.  Returns false — with `g` untouched — for anything else; compact_step decides then.
-template <int R>
+template <int R, typename Off = uint32_t>
 __device__ __forceinline__ bool compact_hot_step(CGroup<R> &g, const uint32_t flag, const uint32_t (&wb)[R > 1 ? R - 1 : 1],
                                                  const uint32_t nprop, const uint32_t gate, const uint32_t et, const uint32_t ht,
                                                  uint32_t &out, uint32_t &adv, uint32_t &dirty) {
@@ -1210,7 +1224,7 @@ __device__ __forceinline__ bool compact_hot_step(CGroup<R> &g, const uint32_t fl
   bool hot = (flag & (CF_COMPACT | CF_TERM_OK)) == (CF_COMPACT | CF_TERM_OK) &&
              (g.meta & kSettled) == ((uint64_t)MRQ_ROLE_LEADER | (1ull << 63));
   uint32_t li = g.m[R - 1];
-  hot = hot && li + nprop <= kCompactSpan;
+  hot = hot && li + nprop <= compact_span<Off>();
   uint32_t nm[R];
   uint32_t d = 0, min_ack = MRQ_P8_NO_ACK, kinds = 0, mx_max = 0, moved = 0;
 #pragma unroll
@@ -1284,7 +1298,7 @@ __device__ __forceinline__ bool compact_hot_step(CGroup<R> &g, const uint32_t fl
 // One tick of one group on compact state, every case the compact form can express.  Returns true (and leaves `g`
 // untouched) when the group needs the general path.  `wb[j]`: the frame's byte of row j, `nprop`: the proposal byte,
 // `gate`: c.gate of the group (only looked at while CF_GATE_OPEN is clear).  Mirrors fast_group_tick8 in offset space.
-template <int R>
+template <int R, typename Off = uint32_t>
 __device__ __forceinline__ bool compact_step(CGroup<R> &g, const uint32_t flag, const uint32_t (&wb)[R > 1 ? R - 1 : 1],
                                              const uint32_t nprop, const uint32_t gate, const uint32_t et, const uint32_t ht,
                                              uint32_t &out, uint32_t &adv, uint32_t &dirty) {
@@ -1316,7 +1330,7 @@ __device__ __forceinline__ bool compact_step(CGroup<R> &g, const uint32_t flag, 
   if (m.role == MRQ_ROLE_LEADER) {
     if (m.strict || !m.ltok || any_hb) return true;
     if (any_ack && !(flag & CF_TERM_OK)) return true;
-    if (li + nprop > kCompactSpan) return true;  // time to re-base
+    if (li + nprop > compact_span<Off>()) return true;  // time to re-base
     bool changed = false;
 #pragma unroll
     for (int j = 0; j < R - 1; ++j)
@@ -1390,7 +1404,8 @@ __device__ __forceinline__ bool compact_step(CGroup<R> &g, const uint32_t flag, 
 }
 
 // compact -> wide for one group: the wide columns become exact copies (flag untouched)
-__device__ __forceinline__ void materialise_group(const StateView &s, const CompactView &c, uint64_t *base_index, uint64_t gs, uint32_t R,
+template <typename Off>
+__device__ __forceinline__ void materialise_group(const StateView &s, const CompactViewT<Off> &c, uint64_t *base_index, uint64_t gs, uint32_t R,
                                                   const uint64_t i) {
   if (!(c.flag[i] & CF_COMPACT)) return;
   const Meta m = meta_unpack(s.meta[i]);
@@ -1409,14 +1424,15 @@ __device__ __forceinline__ void materialise_group(const StateView &s, const Comp
 
 // wide -> compact for one group (after the general path, an import, or a new window base): picks a fresh ibase just
 // below min(committed, window base) and writes the offsets; a group that does not fit stays wide (flag 0)
-__device__ __forceinline__ void compact_group(const StateView &s, const CompactView &c, const uint64_t *base_index,
+template <typename Off>
+__device__ __forceinline__ void compact_group(const StateView &s, const CompactViewT<Off> &c, const uint64_t *base_index,
                                               const uint64_t *base_term, uint64_t gs, uint32_t R, const uint64_t i) {
   const Meta m = meta_unpack(s.meta[i]);
   const uint64_t li = s.last_index[i], cm = s.committed[i], wb = base_index[i], gate = s.term_start[i];
   const uint64_t lo = cm < wb ? cm : wb;
   const uint64_t ib = lo ? lo - 1u : 0u;
-  bool fits = m.self >= 1 && m.self <= R && !m.strict && cm <= li && li - ib <= (uint64_t)kCompactSpan &&
-              wb - ib <= (uint64_t)kCompactSpan;
+  const uint64_t span = compact_span<Off>();
+  bool fits = m.self >= 1 && m.self <= R && !m.strict && cm <= li && li - ib <= span && wb - ib <= span;
   const bool leader = m.role == MRQ_ROLE_LEADER;
   if (fits && leader) fits = s.match[(uint64_t)(m.self - 1u) * gs + i] == li;  // a leader's own Match is lastIndex
   if (!fits) {
@@ -1425,19 +1441,20 @@ __device__ __forceinline__ void compact_group(const StateView &s, const CompactV
   }
   c.ibase[i] = ib;
   c.iblo[i] = (uint32_t)ib;
-  c.commit[i] = (uint32_t)(cm - ib);
-  c.win[i] = (uint32_t)(wb - ib);
+  c.commit[i] = (Off)(cm - ib);
+  c.win[i] = (Off)(wb - ib);
   for (uint32_t j = 0; j + 1u < R; ++j) {
-    uint32_t v = 0;
+    Off v = 0;
     if (leader) {
       const uint64_t mv = s.match[(uint64_t)crow_sender(j, m.self) * gs + i];
-      v = mv > ib ? (uint32_t)(mv - ib) : 0u;  // mv <= lastIndex (not strict), so the offset fits
+      v = mv > ib ? (Off)(mv - ib) : (Off)0;  // mv <= lastIndex (not strict), so the offset fits
     }
     c.match[(uint64_t)j * gs + i] = v;
   }
-  c.match[(uint64_t)(R - 1u) * gs + i] = (uint32_t)(li - ib);
-  uint32_t go = 0xFFFFFFFFu;  // closed for good (not a leader)
-  if (leader) go = gate > ib ? (gate - ib > 0xFFFFFFFEull ? 0xFFFFFFFFu : (uint32_t)(gate - ib)) : 0u;
+  c.match[(uint64_t)(R - 1u) * gs + i] = (Off)(li - ib);
+  constexpr Off kClosed = static_cast<Off>(~Off(0));  // closed for good: above every offset the span allows
+  Off go = kClosed;  // (not a leader)
+  if (leader) go = gate > ib ? (gate - ib >= (uint64_t)kClosed ? kClosed : (Off)(gate - ib)) : (Off)0;
   c.gate[i] = go;
   c.flag[i] = (uint8_t)(CF_COMPACT | (base_term[i] == s.term[i] ? CF_TERM_OK : 0u) | ((leader && gate <= cm) ? CF_GATE_OPEN : 0u));
 }
@@ -1451,9 +1468,10 @@ struct TickDesc {
   uint8_t *delta;        // [gs] this tick's commit advances, saturating at 255 ("read the index in full")
 };
 static constexpr uint32_t kMaxTicksPerLaunch = 96;  // descriptors of one launch live in shared memory (96 x 88 B)
-struct Tick4Args {
+template <typename Off = uint32_t>
+struct Tick4ArgsT {
   TickArgs t;  // t.in and t.s.out are per tick (TickDesc)
-  CompactView c;
+  CompactViewT<Off> c;
   uint64_t *base_index;  // the wide window base (general path only)
   const uint64_t *base_term;
   TickDesc d0;            // nticks == 1: the descriptor rides in the kernel arguments
@@ -1462,10 +1480,11 @@ struct Tick4Args {
   uint32_t write_through;  // nticks > 1: 1 = the state columns are written after every tick, 0 = after the last one
   unsigned long long *slow_list64;  // (first general tick << 32) | group
 };
+using Tick4Args = Tick4ArgsT<>;
 
 // The general path of mode 4 for one group, from tick t0 of the launch to its last tick.
-template <int R>
-__device__ __forceinline__ uint32_t slow_group_ticks_c(const Tick4Args &A, const uint64_t i, const uint32_t t0) {
+template <int R, typename Off>
+__device__ __forceinline__ uint32_t slow_group_ticks_c(const Tick4ArgsT<Off> &A, const uint64_t i, const uint32_t t0) {
   const TickArgs &a0 = A.t;
   materialise_group(a0.s, A.c, A.base_index, a0.gs, (uint32_t)R, i);
   uint32_t ev = 0;
@@ -1501,14 +1520,14 @@ __device__ __noinline__ CStepResult<R> compact_step_cold(CGroup<R> g, uint32_t f
 #pragma unroll
   for (int j = 0; j < (R > 1 ? R - 1 : 1); ++j) wb[j] = ((j < 4 ? w0123 : w4567) >> (8 * (j & 3))) & 0xFFu;  // the group's R-1 bytes, packed
   CStepResult<R> r;
-  r.slow = compact_step<R>(g, flag, wb, nprop, gate, et, ht, r.out, r.adv, r.dirty) ? 1u : 0u;
+  r.slow = compact_step<R, CompactOff>(g, flag, wb, nprop, gate, et, ht, r.out, r.adv, r.dirty) ? 1u : 0u;
   r.g = g;
   return r;
 }
 #endif
 
 #ifndef MRQ_HOST_EMULATION
-// 128-bit column accesses with the L2 residency policy of the scalar kernels
+// Vector column accesses with the L2 residency policy of the scalar kernels
 struct u32x4 {
   uint32_t v[4];
 };
@@ -1530,6 +1549,25 @@ __device__ __forceinline__ void ld_v2u64_p(const uint64_t *p, uint64_t pol, uint
 __device__ __forceinline__ void st_v2u64_p(uint64_t *p, uint64_t a, uint64_t b, uint64_t pol) {
   asm volatile("st.global.L1::no_allocate.L2::cache_hint.v2.u64 [%0], {%1, %2}, %3;" ::"l"(p), "l"(a), "l"(b), "l"(pol) : "memory");
 }
+// The 16-bit offset columns: a quad is one 64-bit access, widened to u32 at the load and narrowed at the store
+__device__ __forceinline__ u32x4 ld_v4u16_p(const uint16_t *p, uint64_t pol) {
+  uint32_t a, b;
+  asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v2.u32 {%0, %1}, [%2], %3;" : "=r"(a), "=r"(b) : "l"(p), "l"(pol));
+  return u32x4{{__byte_perm(a, 0u, 0x4410), __byte_perm(a, 0u, 0x4432), __byte_perm(b, 0u, 0x4410), __byte_perm(b, 0u, 0x4432)}};
+}
+__device__ __forceinline__ void st_v4u16_p(uint16_t *p, const u32x4 &r, uint64_t pol) {
+  asm volatile("st.global.L1::no_allocate.L2::cache_hint.v2.u32 [%0], {%1, %2}, %3;" ::"l"(p), "r"(__byte_perm(r.v[0], r.v[1], 0x5410)),
+               "r"(__byte_perm(r.v[2], r.v[3], 0x5410)), "l"(pol)
+               : "memory");
+}
+__device__ __forceinline__ uint32_t ld_stream_u16_p(const uint16_t *p, uint64_t pol) {
+  uint32_t v;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u16 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ void st_state_u16_p(uint16_t *p, uint32_t v, uint64_t pol) {
+  asm volatile("st.global.L1::no_allocate.L2::cache_hint.u16 [%0], %1, %2;" ::"l"(p), "r"(v), "l"(pol) : "memory");
+}
 
 // THREADS x 4 groups per CTA.  128 for big shards; a shard of a many-GPU job is too small to fill 132 SMs with 512-group
 // CTAs (131,072 groups = 256 of them), so the host picks 64 or 32 threads there: same register budget per SM, more CTAs.
@@ -1537,7 +1575,7 @@ template <int R, int THREADS>
 #ifndef MRQ_T4_THREADS_PER_SM
 #define MRQ_T4_THREADS_PER_SM 512  // resident threads per SM the register budget is cut for (development knob)
 #endif
-__global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384) / THREADS) tick_fast4_kernel(const Tick4Args A) {
+__global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384) / THREADS) tick_fast4_kernel(const Tick4ArgsT<CompactOff> A) {
   const TickArgs &a = A.t;
   pdl_launch_dependents();
   const uint64_t i0 = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4u;
@@ -1554,11 +1592,11 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
     const uint32_t fw = ld_stream_u32_p(reinterpret_cast<const uint32_t *>(A.c.flag + i), pol_keep);
     ld_v2u64_p(a.s.meta + i, pol_keep, g[0].meta, g[1].meta);
     ld_v2u64_p(a.s.meta + i + 2, pol_keep, g[2].meta, g[3].meta);
-    const u32x4 cm = ld_v4u32_p(A.c.commit + i, pol_keep);
-    const u32x4 wn = ld_v4u32_p(A.c.win + i, pol_keep);
+    const u32x4 cm = ld_v4u16_p(A.c.commit + i, pol_keep);
+    const u32x4 wn = ld_v4u16_p(A.c.win + i, pol_keep);
     u32x4 mv[R];
 #pragma unroll
-    for (int r = 0; r < R; ++r) mv[r] = ld_v4u32_p(A.c.match + (uint64_t)r * a.gs + i, pol_keep);
+    for (int r = 0; r < R; ++r) mv[r] = ld_v4u16_p(A.c.match + (uint64_t)r * a.gs + i, pol_keep);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       flag[k] = (fw >> (8 * k)) & 0xFFu;
@@ -1573,7 +1611,7 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
   for (int k = 0; k < 4; ++k)
     if (!active || i0 + k >= a.G) stopped |= 1u << k;
   u32x4 gate{};  // only the few groups whose commit gate is still closed look at it
-  if (((flag[0] & flag[1] & flag[2] & flag[3]) & CF_GATE_OPEN) == 0u) gate = ld_v4u32_p(A.c.gate + i, pol_keep);
+  if (((flag[0] & flag[1] & flag[2] & flag[3]) & CF_GATE_OPEN) == 0u) gate = ld_v4u16_p(A.c.gate + i, pol_keep);
   const bool gather = a.world > 1;
   u32x4 iblo{};
   if (gather) iblo = ld_v4u32_p(A.c.iblo + i, pol_keep);
@@ -1624,7 +1662,7 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
       uint32_t o, adv, dirty;
       const uint32_t np = (pb >> (8 * k)) & 0xFFu;
       bool slow = false;
-      if (!compact_hot_step<R>(g[k], flag[k], wk, np, gate.v[k], a.election_tick, a.heartbeat_tick, o, adv, dirty)) {
+      if (!compact_hot_step<R, CompactOff>(g[k], flag[k], wk, np, gate.v[k], a.election_tick, a.heartbeat_tick, o, adv, dirty)) {
         uint32_t p0 = 0, p1 = 0;  // the group's bytes, four to a word
 #pragma unroll
         for (int j = 0; j < R - 1; ++j) {
@@ -1700,7 +1738,7 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
         }
       }
     }
-    // ---- state write-back: per warp, whole 16-byte quads (see fast_group_tick for why per warp) ---------------------
+    // ---- state write-back: per warp, whole quads (see fast_group_tick for why per warp) -----------------------------
     const bool last = t + 1 == A.nticks;
     if (A.write_through || last) {
       uint32_t wd = __reduce_or_sync(0xFFFFFFFFu, A.write_through ? tdirty : acc_dirty);
@@ -1709,12 +1747,12 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
           st_v2u64_p(a.s.meta + i, g[0].meta, g[1].meta, pol_keep);
           st_v2u64_p(a.s.meta + i + 2, g[2].meta, g[3].meta, pol_keep);
         }
-        if (wd & CD_COMMIT) st_v4u32_p(A.c.commit + i, u32x4{{g[0].commit, g[1].commit, g[2].commit, g[3].commit}}, pol_keep);
-        if (wd & CD_WIN) st_v4u32_p(A.c.win + i, u32x4{{g[0].win, g[1].win, g[2].win, g[3].win}}, pol_keep);
+        if (wd & CD_COMMIT) st_v4u16_p(A.c.commit + i, u32x4{{g[0].commit, g[1].commit, g[2].commit, g[3].commit}}, pol_keep);
+        if (wd & CD_WIN) st_v4u16_p(A.c.win + i, u32x4{{g[0].win, g[1].win, g[2].win, g[3].win}}, pol_keep);
         if (wd & CD_MATCH_ANY) {
 #pragma unroll
           for (int r = 0; r < R; ++r)
-            st_v4u32_p(A.c.match + (uint64_t)r * a.gs + i, u32x4{{g[0].m[r], g[1].m[r], g[2].m[r], g[3].m[r]}}, pol_keep);
+            st_v4u16_p(A.c.match + (uint64_t)r * a.gs + i, u32x4{{g[0].m[r], g[1].m[r], g[2].m[r], g[3].m[r]}}, pol_keep);
         }
       }
     }
@@ -1736,7 +1774,7 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
 // walks ~800 dependent instructions per tick alone on its scheduler, and that chain sets a small shard's floor).
 // Scalar column accesses — the bytes no longer matter at this size, the number of warps in flight does.
 template <int R>
-__global__ void __launch_bounds__(128, 7) tick_fast1_kernel(const Tick4Args A) {
+__global__ void __launch_bounds__(128, 7) tick_fast1_kernel(const Tick4ArgsT<CompactOff> A) {
   const TickArgs &a = A.t;
   pdl_launch_dependents();
   const uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1757,11 +1795,11 @@ __global__ void __launch_bounds__(128, 7) tick_fast1_kernel(const Tick4Args A) {
   CGroup<R> g;
   const uint32_t flag = ld_stream_u8_p(A.c.flag + i, pol_keep);
   g.meta = ld_state_p(a.s.meta + i, pol_keep);
-  g.commit = ld_stream_u32_p(A.c.commit + i, pol_keep);
-  g.win = ld_stream_u32_p(A.c.win + i, pol_keep);
+  g.commit = ld_stream_u16_p(A.c.commit + i, pol_keep);
+  g.win = ld_stream_u16_p(A.c.win + i, pol_keep);
 #pragma unroll
-  for (int r = 0; r < R; ++r) g.m[r] = ld_stream_u32_p(A.c.match + (uint64_t)r * a.gs + i, pol_keep);
-  const uint32_t gate = (flag & CF_GATE_OPEN) ? 0u : ld_stream_u32_p(A.c.gate + i, pol_keep);
+  for (int r = 0; r < R; ++r) g.m[r] = ld_stream_u16_p(A.c.match + (uint64_t)r * a.gs + i, pol_keep);
+  const uint32_t gate = (flag & CF_GATE_OPEN) ? 0u : ld_stream_u16_p(A.c.gate + i, pol_keep);
   const bool gather = a.world > 1;
   const uint32_t iblo = gather ? ld_stream_u32_p(A.c.iblo + i, pol_keep) : 0u;
   constexpr int NW = R > 1 ? R - 1 : 1;
@@ -1792,7 +1830,7 @@ __global__ void __launch_bounds__(128, 7) tick_fast1_kernel(const Tick4Args A) {
     bool newly = false;
     const uint32_t lo_old = iblo + g.commit;
     if (!stopped) {
-      if (!compact_hot_step<R>(g, flag, wb, pb, gate, a.election_tick, a.heartbeat_tick, o, adv, dirty)) {
+      if (!compact_hot_step<R, CompactOff>(g, flag, wb, pb, gate, a.election_tick, a.heartbeat_tick, o, adv, dirty)) {
         uint32_t p0 = 0, p1 = 0;
 #pragma unroll
         for (int j = 0; j < R - 1; ++j) {
@@ -1858,11 +1896,11 @@ __global__ void __launch_bounds__(128, 7) tick_fast1_kernel(const Tick4Args A) {
       const uint32_t wd = __reduce_or_sync(0xFFFFFFFFu, A.write_through ? dirty : acc_dirty);
       if (valid) {
         if (wd & CD_META) st_state_p(a.s.meta + i, g.meta, pol_keep);
-        if (wd & CD_COMMIT) st_state_u32_p(A.c.commit + i, g.commit, pol_keep);
-        if (wd & CD_WIN) st_state_u32_p(A.c.win + i, g.win, pol_keep);
+        if (wd & CD_COMMIT) st_state_u16_p(A.c.commit + i, g.commit, pol_keep);
+        if (wd & CD_WIN) st_state_u16_p(A.c.win + i, g.win, pol_keep);
         if (wd & CD_MATCH_ANY) {
 #pragma unroll
-          for (int r = 0; r < R; ++r) st_state_u32_p(A.c.match + (uint64_t)r * a.gs + i, g.m[r], pol_keep);
+          for (int r = 0; r < R; ++r) st_state_u16_p(A.c.match + (uint64_t)r * a.gs + i, g.m[r], pol_keep);
         }
       }
     }
@@ -1880,7 +1918,7 @@ __global__ void __launch_bounds__(128, 7) tick_fast1_kernel(const Tick4Args A) {
 }
 
 template <int R>
-__global__ void __launch_bounds__(kTickThreads, (R <= 5 ? 6 : 5)) tick_slow4_kernel(const Tick4Args A) {
+__global__ void __launch_bounds__(kTickThreads, (R <= 5 ? 6 : 5)) tick_slow4_kernel(const Tick4ArgsT<CompactOff> A) {
   const TickArgs &a = A.t;
   pdl_launch_dependents();
   pdl_wait();
@@ -1900,14 +1938,14 @@ __global__ void __launch_bounds__(kTickThreads, (R <= 5 ? 6 : 5)) tick_slow4_ker
 }
 
 // whole-engine passes between the two representations (import / export / a new window base / a mode switch)
-__global__ void __launch_bounds__(256) materialise_all_kernel(StateView s, CompactView c, uint64_t *base_index, uint64_t gs, uint64_t G,
+__global__ void __launch_bounds__(256) materialise_all_kernel(StateView s, CompactViewT<CompactOff> c, uint64_t *base_index, uint64_t gs, uint64_t G,
                                                                uint32_t R, int clear_flags) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= G) return;
   materialise_group(s, c, base_index, gs, R, i);
   if (clear_flags) c.flag[i] = 0;
 }
-__global__ void __launch_bounds__(256) compact_all_kernel(StateView s, CompactView c, const uint64_t *base_index,
+__global__ void __launch_bounds__(256) compact_all_kernel(StateView s, CompactViewT<CompactOff> c, const uint64_t *base_index,
                                                            const uint64_t *base_term, uint64_t gs, uint64_t G, uint32_t R) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= G) return;
