@@ -59,9 +59,17 @@ tests/cpp/tick_host16_test: $(TICKHOST16_DEP)
 	$(CXX) -std=c++17 -O1 -I$(CUDA_INC) -pthread -o $@ $(TICKHOST16_SRC)
 tests/cpp/tick_host16_test_san: $(TICKHOST16_DEP)
 	$(SAN_CXX) -std=c++17 -O0 -fsanitize=address,undefined -fno-sanitize-recover=undefined -I$(CUDA_INC) -pthread -o $@ $(TICKHOST16_SRC)
+# The library's form: 16-bit offsets and clock-relative leader timers (it includes tick_host_test.cpp for the harness).
+TICKCLOCK_SRC := tests/cpp/tick_clock_host_test.cpp oracle/raft_oracle.c
+TICKCLOCK_DEP := $(TICKCLOCK_SRC) $(TICKHOST_DEP)
+tests/cpp/tick_clock_host_test: $(TICKCLOCK_DEP)
+	$(CXX) -std=c++17 -O1 -I$(CUDA_INC) -pthread -o $@ $(TICKCLOCK_SRC)
+tests/cpp/tick_clock_host_test_san: $(TICKCLOCK_DEP)
+	$(SAN_CXX) -std=c++17 -O0 -fsanitize=address,undefined -fno-sanitize-recover=undefined -I$(CUDA_INC) -pthread -o $@ $(TICKCLOCK_SRC)
 
 clean:
 	rm -f $(LIB) $(HOSTLIB) $(CPPTEST) tests/cpp/raftpipe_test_asan tests/cpp/raftpipe_test_tsan build_ptxas.log \
-	  tests/cpp/tick_host_test tests/cpp/tick_host_test_san tests/cpp/tick_host16_test tests/cpp/tick_host16_test_san
+	  tests/cpp/tick_host_test tests/cpp/tick_host_test_san tests/cpp/tick_host16_test tests/cpp/tick_host16_test_san \
+	  tests/cpp/tick_clock_host_test tests/cpp/tick_clock_host_test_san
 	$(MAKE) -C oracle clean
 .PHONY: all oracle clean san_cxx

@@ -383,7 +383,11 @@ int mrq_ipc_export(mrq_engine *e, uint8_t handle_out[MRQ_IPC_HANDLE_BYTES]);
 int mrq_ipc_attach(mrq_engine *e, const uint8_t *handles, uint32_t rank, uint32_t world);
 
 /* ---- raw device pointers (zero-copy integration with a host that already lives on the GPU;
- * also lets tests / torch wrap the buffers).  `which` is an MRQ_PTR_* id.                    */
+ * also lets tests / torch wrap the buffers).  `which` is an MRQ_PTR_* id.
+ * In tick mode 4 some raw columns are exact only in the wide representation, i.e. right after a call
+ * that converts (an export, mrq_sync_commits, ...): COMMITTED, LAST_INDEX and MATCH (kept as offsets
+ * from a per-group base), and META's electionElapsed / heartbeatElapsed fields of a leader (kept as
+ * phases against the tick number).                                                              */
 #define MRQ_PTR_TERM 0
 #define MRQ_PTR_META 1
 #define MRQ_PTR_LAST_INDEX 2

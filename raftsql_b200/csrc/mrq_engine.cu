@@ -252,6 +252,7 @@ int ensure_compact_alloc(mrq_engine *e) {
   if ((r = dalloc(e, &e->c.iblo, gs))) return r;
   if ((r = dalloc(e, &e->c.match, gs * e->R))) return r;
   if ((r = dalloc(e, &e->c.ibase, gs))) return r;
+  if ((r = dalloc(e, &e->c.clk, gs))) return r;
   if ((r = dalloc(e, &e->slow_list64, gs))) return r;
   e->compact_alloc = true;
   return MRQ_OK;
@@ -261,7 +262,8 @@ int ensure_compact_alloc(mrq_engine *e) {
 // wide state, so the compact copies die (every group is re-compacted by the next mode-4 tick).
 int ensure_wide(mrq_engine *e, bool invalidate) {
   if (!e->compact_live || e->G == 0) return MRQ_OK;
-  materialise_all_kernel<<<nblocks(e->G), 256, 0, e->stream>>>(e->s, e->c, e->pk_base_index, e->gs, e->G, e->R, invalidate ? 1 : 0);
+  materialise_all_kernel<<<nblocks(e->G), 256, 0, e->stream>>>(e->s, e->c, e->pk_base_index, e->gs, e->G, e->R, invalidate ? 1 : 0,
+                                                               e->tick_no, e->cfg.election_tick, e->cfg.heartbeat_tick);
   CK(e, cudaGetLastError());
   e->launches++;
   if (invalidate) e->compact_live = false;
@@ -272,7 +274,8 @@ int ensure_compact(mrq_engine *e) {
   if (e->compact_live || e->G == 0) return MRQ_OK;
   int r = ensure_compact_alloc(e);
   if (r) return r;
-  compact_all_kernel<<<nblocks(e->G), 256, 0, e->stream>>>(e->s, e->c, e->pk_base_index, e->pk_base_term, e->gs, e->G, e->R);
+  compact_all_kernel<<<nblocks(e->G), 256, 0, e->stream>>>(e->s, e->c, e->pk_base_index, e->pk_base_term, e->gs, e->G, e->R, e->tick_no,
+                                                           e->cfg.election_tick, e->cfg.heartbeat_tick);
   CK(e, cudaGetLastError());
   e->launches++;
   e->compact_live = true;
@@ -305,6 +308,10 @@ void fill_tick_args(mrq_engine *e, TickArgs &a) {
 
 // n ticks of mode 4 in ONE pair of launches: every slot holds a byte frame (mrq_post_inbox_packed, word_bits 8).
 int launch_tick4(mrq_engine *e, const uint32_t *slots, uint32_t n) {
+  // compact leaders' timers are phases against the tick number, which must not wrap within the compact representation
+  if (n > UINT64_MAX - e->tick_no)
+    return fail(e, MRQ_E_INVAL, "tick mode 4: tick number %llu + %u would wrap past 2^64 - 1 (rewind it with mrq_set_tick_count)",
+                (unsigned long long)e->tick_no, n);
   int r = ensure_compact(e);
   if (r) return r;
   Tick4ArgsT<CompactOff> A{};
@@ -681,7 +688,7 @@ void mrq_destroy(mrq_engine *e) {
   for (auto &kv : e->graphs) cudaGraphExecDestroy(kv.second);
   for (auto &kv : e->desc_tables) cudaFree(kv.second);
   {
-    void *cp[] = {e->c.flag, e->c.commit, e->c.win, e->c.gate, e->c.iblo, e->c.match, e->c.ibase, e->slow_list64};
+    void *cp[] = {e->c.flag, e->c.commit, e->c.win, e->c.gate, e->c.iblo, e->c.match, e->c.ibase, e->c.clk, e->slow_list64};
     for (void *p : cp)
       if (p) cudaFree(p);
     for (void *p : e->out_slot)
@@ -707,6 +714,9 @@ uint64_t mrq_tick_count(const mrq_engine *e) { return e ? e->tick_no : 0; }
 int mrq_set_tick_count(mrq_engine *e, uint64_t t) {
   if (!e) return MRQ_E_INVAL;
   CK(e, cudaSetDevice(e->device));
+  // compact leaders keep their timers as phases against the tick number: bring them into meta before it moves
+  int r = ensure_wide(e, true);
+  if (r) return r;
   e->tick_no = t;
   // also normalise the double-buffer parities, so that a slot sequence replayed after a rewind hits the
   // same captured graph (mrq_tick_many keys its graphs by parity)

@@ -1161,7 +1161,8 @@ __global__ void __launch_bounds__(kTickThreads, (R <= 5 ? 6 : 5)) tick_general_k
 //                         CF_GATE_OPEN (leader, term_start <= committed: the commit gate can no longer block)
 // term, term_start, last_term never change on the fast path: they stay wide and are never read by it.  With the byte
 // inbox (R-1 sender bytes + 1 proposal byte) the steady-state tick reads 8 (meta) + 1 + 2 + 2 + 2R + R = 28 B and
-// writes 8 + 4 (out) + 1 (commit advance) + 2 + 2 + 2(R-1) + 1.5 = 26.5 B per group at R = 5: 54.5 B instead of 217.
+// writes 4 (out) + 1 (commit advance) + 2 + 2 + 2(R-1) + 1.5 = 18.5 B per group at R = 5: 46.5 B instead of 217 (a
+// leader's timers run on the clock, c.clk below, so its meta word is not rewritten).
 // One thread owns FOUR adjacent groups: every column access is one 64-bit (u16 x 4), 128-bit (u32 x 4) or two 128-bit
 // (u64 x 4) loads or stores, which also cuts the instruction count per group-tick to a quarter of the scalar kernels'.
 // Sixteen bits hold ~43k ticks of log growth at the steady trace's 1.5 proposals per tick; a group that outgrows
@@ -1196,8 +1197,26 @@ struct CompactViewT {
   uint32_t *iblo;   // [gs] low word of ibase (fused gather only)
   Off *match;       // [R][gs]
   uint64_t *ibase;  // [gs]
+  uint32_t *clk;    // [gs] a compact leader's timer phases (see clk_phase); null: its timers stay in meta
 };
 using CompactView = CompactViewT<>;
+
+// Clock-relative timers.  On a compact leader's tick both timers are pure clocks — electionElapsed goes to
+// (el + 1) mod ElectionTick (checkQuorum is off, nothing else reads or resets it) and heartbeatElapsed to
+// (hb + 1) mod HeartbeatTick — so, like the indices against ibase, they are stored against the engine's tick number T
+// (the number of the next tick to run): c.clk holds p_el = (el - T) mod ET in bits [0,16) and p_hb = (hb - T) mod HT
+// in bits [16,24), and the timers before tick T are (p + T) mod ET / HT.  The phases never change while the group
+// stays a compact leader, so the batched tick neither stores them nor the meta word for it; meta's two timer fields
+// are not the truth for such a group, as the wide committed / match columns are not.  Anything that changes role or
+// term runs on the general path, which materialises the real timers into meta first.
+__host__ __device__ __forceinline__ uint32_t clk_phase(uint32_t v, uint64_t T, uint32_t m) {  // (v - T) mod m, v < m
+  const uint32_t tm = (uint32_t)(T % m);
+  return v >= tm ? v - tm : v + m - tm;
+}
+__host__ __device__ __forceinline__ uint32_t clk_value(uint32_t p, uint64_t T, uint32_t m) {  // (p + T) mod m, p < m
+  const uint32_t s = p + (uint32_t)(T % m);
+  return s >= m ? s - m : s;
+}
 
 template <int R>
 struct CGroup {  // one group's compact state, in registers
@@ -1214,15 +1233,21 @@ __host__ __device__ __forceinline__ uint32_t crow_sender(uint32_t j, uint32_t se
   return j + (j + 1u >= self_id ? 1u : 0u);
 }
 
-// The HOT case of a tick, straight-line: a settled leader (no strict mode, lastTerm == Term) whose frame holds nothing
-// but in-window acks of its own term.  Returns false — with `g` untouched — for anything else; compact_step decides then.
-template <int R, typename Off = uint32_t>
-__device__ __forceinline__ bool compact_hot_step(CGroup<R> &g, const uint32_t flag, const uint32_t (&wb)[R > 1 ? R - 1 : 1],
-                                                 const uint32_t nprop, const uint32_t gate, const uint32_t et, const uint32_t ht,
-                                                 uint32_t &out, uint32_t &adv, uint32_t &dirty) {
+// A settled leader: compact, its window messages carry its term, no strict mode, lastTerm == Term.  Only the general
+// path changes role, strict, ltok or the flag, and a group that takes it leaves the fast kernels for the rest of the
+// launch, so the answer holds for a whole launch.
+__device__ __forceinline__ bool compact_settled(const uint32_t flag, const uint64_t meta) {
   constexpr uint64_t kSettled = 3ull | (1ull << 62) | (1ull << 63);  // role, strict, ltok
-  bool hot = (flag & (CF_COMPACT | CF_TERM_OK)) == (CF_COMPACT | CF_TERM_OK) &&
-             (g.meta & kSettled) == ((uint64_t)MRQ_ROLE_LEADER | (1ull << 63));
+  return (flag & (CF_COMPACT | CF_TERM_OK)) == (CF_COMPACT | CF_TERM_OK) &&
+         (meta & kSettled) == ((uint64_t)MRQ_ROLE_LEADER | (1ull << 63));
+}
+
+// The HOT case of a tick, straight-line: a settled leader whose frame holds nothing but in-window acks of its own term.
+// This part does the acks, the proposals, the commit and the window; the callers below add the timers.  Returns false
+// — with `g` untouched — for anything else; compact_step decides then.
+template <int R, typename Off>
+__device__ __forceinline__ bool compact_hot_log(CGroup<R> &g, bool hot, const uint32_t flag, const uint32_t (&wb)[R > 1 ? R - 1 : 1],
+                                                const uint32_t nprop, const uint32_t gate, uint32_t &out, uint32_t &adv, uint32_t &dirty) {
   uint32_t li = g.m[R - 1];
   hot = hot && li + nprop <= compact_span<Off>();
   uint32_t nm[R];
@@ -1263,6 +1288,26 @@ __device__ __forceinline__ bool compact_hot_step(CGroup<R> &g, const uint32_t fl
     d |= CD_COMMIT;
     o |= MRQ_OUT_COMMIT_ADVANCED | MRQ_OUT_BCAST_APPEND;
   }
+  if (min_ack < MRQ_P8_NO_ACK && min_ack > MRQ_P8_SLACK) {  // the window slides for whoever decodes the frame
+    g.win += min_ack - MRQ_P8_SLACK;
+    d |= CD_WIN;
+  }
+  g.commit = commit;
+#pragma unroll
+  for (int r = 0; r < R; ++r) g.m[r] = nm[r];
+  out = o;
+  adv = q;
+  dirty = d;
+  return true;
+}
+
+// The hot step with the timers in meta (c.clk null).
+template <int R, typename Off = uint32_t>
+__device__ __forceinline__ bool compact_hot_step(CGroup<R> &g, const uint32_t flag, const uint32_t (&wb)[R > 1 ? R - 1 : 1],
+                                                 const uint32_t nprop, const uint32_t gate, const uint32_t et, const uint32_t ht,
+                                                 uint32_t &out, uint32_t &adv, uint32_t &dirty) {
+  uint32_t o, d;
+  if (!compact_hot_log<R, Off>(g, compact_settled(flag, g.meta), flag, wb, nprop, gate, o, adv, d)) return false;
   // tickHeartbeat on the packed word: electionElapsed bits [14,26), heartbeatElapsed bits [38,46)
   uint32_t lo = (uint32_t)g.meta, hi = (uint32_t)(g.meta >> 32);
   uint32_t el = ((lo >> 14) & 0xFFFu) + 1u;
@@ -1281,27 +1326,41 @@ __device__ __forceinline__ bool compact_hot_step(CGroup<R> &g, const uint32_t fl
   }
   const uint64_t nmeta = ((uint64_t)hi << 32) | lo;
   d |= nmeta != g.meta ? CD_META : 0u;
-  if (min_ack < MRQ_P8_NO_ACK && min_ack > MRQ_P8_SLACK) {  // the window slides for whoever decodes the frame
-    g.win += min_ack - MRQ_P8_SLACK;
-    d |= CD_WIN;
-  }
   g.meta = nmeta;
-  g.commit = commit;
-#pragma unroll
-  for (int r = 0; r < R; ++r) g.m[r] = nm[r];
   out = o;
-  adv = q;
   dirty = d;
+  return true;
+}
+
+// The hot step with clock-relative timers (c.clk): `settled` is compact_settled() of the group, evaluated once per
+// launch, and its heartbeatElapsed is the byte at bit `shift` of `hbw`, a countdown kept in registers (only looked at
+// when HeartbeatTick > 1).  The election timer needs no work at all, and neither meta nor c.clk changes.
+template <int R, typename Off>
+__device__ __forceinline__ bool compact_hot_step_clk(CGroup<R> &g, const bool settled, const uint32_t flag,
+                                                     const uint32_t (&wb)[R > 1 ? R - 1 : 1], const uint32_t nprop, const uint32_t gate,
+                                                     const uint32_t ht, uint32_t &hbw, const uint32_t shift, uint32_t &out, uint32_t &adv,
+                                                     uint32_t &dirty) {
+  if (!compact_hot_log<R, Off>(g, settled, flag, wb, nprop, gate, out, adv, dirty)) return false;
+  if (ht <= 1u) {  // HeartbeatTick 1 (reference raft.go:155; launch-uniform): every tick beats
+    out |= MRQ_OUT_BCAST_HEARTBEAT;
+  } else {
+    uint32_t hb = ((hbw >> shift) & 0xFFu) + 1u;
+    hb = hb >= ht ? 0u : hb;
+    if (hb == 0u) out |= MRQ_OUT_BCAST_HEARTBEAT;
+    hbw = (hbw & ~(0xFFu << shift)) | (hb << shift);
+  }
   return true;
 }
 
 // One tick of one group on compact state, every case the compact form can express.  Returns true (and leaves `g`
 // untouched) when the group needs the general path.  `wb[j]`: the frame's byte of row j, `nprop`: the proposal byte,
 // `gate`: c.gate of the group (only looked at while CF_GATE_OPEN is clear).  Mirrors fast_group_tick8 in offset space.
+// `clk_hb`: null when the timers are in meta; otherwise the timers are clock-relative and *clk_hb is the group's
+// heartbeatElapsed, which a leader's tick advances in place of meta's timer fields (a leader then never sets CD_META).
 template <int R, typename Off = uint32_t>
 __device__ __forceinline__ bool compact_step(CGroup<R> &g, const uint32_t flag, const uint32_t (&wb)[R > 1 ? R - 1 : 1],
                                              const uint32_t nprop, const uint32_t gate, const uint32_t et, const uint32_t ht,
-                                             uint32_t &out, uint32_t &adv, uint32_t &dirty) {
+                                             uint32_t &out, uint32_t &adv, uint32_t &dirty, uint32_t *clk_hb = nullptr) {
   out = 0;
   adv = 0;
   dirty = 0;
@@ -1363,12 +1422,18 @@ __device__ __forceinline__ bool compact_step(CGroup<R> &g, const uint32_t flag, 
         out |= MRQ_OUT_COMMIT_ADVANCED | MRQ_OUT_BCAST_APPEND;
       }
     }
-    ++m.hb;  // tickHeartbeat
-    ++m.elapsed;
-    if (m.elapsed >= et) m.elapsed = 0;
-    if (m.hb >= ht) {
-      m.hb = 0;
-      out |= MRQ_OUT_BCAST_HEARTBEAT;
+    if (clk_hb) {  // tickHeartbeat on the clock: electionElapsed needs no work, heartbeatElapsed is the caller's
+      const uint32_t hb = *clk_hb + 1u >= ht ? 0u : *clk_hb + 1u;
+      if (hb == 0u) out |= MRQ_OUT_BCAST_HEARTBEAT;
+      *clk_hb = hb;
+    } else {
+      ++m.hb;  // tickHeartbeat
+      ++m.elapsed;
+      if (m.elapsed >= et) m.elapsed = 0;
+      if (m.hb >= ht) {
+        m.hb = 0;
+        out |= MRQ_OUT_BCAST_HEARTBEAT;
+      }
     }
   } else if (m.role == MRQ_ROLE_FOLLOWER) {
     if (nprop != 0u || any_ack) return true;
@@ -1403,12 +1468,19 @@ __device__ __forceinline__ bool compact_step(CGroup<R> &g, const uint32_t flag, 
   return false;
 }
 
-// compact -> wide for one group: the wide columns become exact copies (flag untouched)
+// compact -> wide for one group: the wide columns become exact copies (flag and c.clk untouched).  With c.clk, `T` is
+// the number of the next tick to run and a leader's real timers are written into meta.
 template <typename Off>
 __device__ __forceinline__ void materialise_group(const StateView &s, const CompactViewT<Off> &c, uint64_t *base_index, uint64_t gs, uint32_t R,
-                                                  const uint64_t i) {
+                                                  const uint64_t i, const uint64_t T = 0, const uint32_t et = 1, const uint32_t ht = 1) {
   if (!(c.flag[i] & CF_COMPACT)) return;
-  const Meta m = meta_unpack(s.meta[i]);
+  Meta m = meta_unpack(s.meta[i]);
+  if (c.clk && m.role == MRQ_ROLE_LEADER) {
+    const uint32_t p = c.clk[i];
+    m.elapsed = clk_value(p & 0xFFFFu, T, et);
+    m.hb = clk_value((p >> 16) & 0xFFu, T, ht);
+    s.meta[i] = meta_pack(m);
+  }
   const uint64_t ib = c.ibase[i];
   s.committed[i] = ib + c.commit[i];
   base_index[i] = ib + c.win[i];
@@ -1423,10 +1495,14 @@ __device__ __forceinline__ void materialise_group(const StateView &s, const Comp
 }
 
 // wide -> compact for one group (after the general path, an import, or a new window base): picks a fresh ibase just
-// below min(committed, window base) and writes the offsets; a group that does not fit stays wide (flag 0)
+// below min(committed, window base) and writes the offsets; a group that does not fit stays wide (flag 0).  With c.clk,
+// `T` is the number of the next tick to run and a leader's timers become phases against it; a leader whose timers are
+// out of range (an import: el >= ET or hb >= HT) would not follow the modular rule on its next tick, so it stays wide
+// until a general tick has normalised them.
 template <typename Off>
 __device__ __forceinline__ void compact_group(const StateView &s, const CompactViewT<Off> &c, const uint64_t *base_index,
-                                              const uint64_t *base_term, uint64_t gs, uint32_t R, const uint64_t i) {
+                                              const uint64_t *base_term, uint64_t gs, uint32_t R, const uint64_t i, const uint64_t T = 0,
+                                              const uint32_t et = 1, const uint32_t ht = 1) {
   const Meta m = meta_unpack(s.meta[i]);
   const uint64_t li = s.last_index[i], cm = s.committed[i], wb = base_index[i], gate = s.term_start[i];
   const uint64_t lo = cm < wb ? cm : wb;
@@ -1435,10 +1511,12 @@ __device__ __forceinline__ void compact_group(const StateView &s, const CompactV
   bool fits = m.self >= 1 && m.self <= R && !m.strict && cm <= li && li - ib <= span && wb - ib <= span;
   const bool leader = m.role == MRQ_ROLE_LEADER;
   if (fits && leader) fits = s.match[(uint64_t)(m.self - 1u) * gs + i] == li;  // a leader's own Match is lastIndex
+  if (fits && leader && c.clk) fits = m.elapsed < et && m.hb < ht;
   if (!fits) {
     c.flag[i] = 0;
     return;
   }
+  if (leader && c.clk) c.clk[i] = clk_phase(m.elapsed, T, et) | (clk_phase(m.hb, T, ht) << 16);
   c.ibase[i] = ib;
   c.iblo[i] = (uint32_t)ib;
   c.commit[i] = (Off)(cm - ib);
@@ -1486,9 +1564,9 @@ using Tick4Args = Tick4ArgsT<>;
 template <int R, typename Off>
 __device__ __forceinline__ uint32_t slow_group_ticks_c(const Tick4ArgsT<Off> &A, const uint64_t i, const uint32_t t0) {
   const TickArgs &a0 = A.t;
-  materialise_group(a0.s, A.c, A.base_index, a0.gs, (uint32_t)R, i);
-  uint32_t ev = 0;
   const uint64_t tick0 = *a0.tick_cur;
+  materialise_group(a0.s, A.c, A.base_index, a0.gs, (uint32_t)R, i, tick0 + t0, a0.election_tick, a0.heartbeat_tick);
+  uint32_t ev = 0;
   for (uint32_t t = t0; t < A.nticks; ++t) {
     const TickDesc d = A.descs ? A.descs[t] : A.d0;
     TickArgs a = a0;
@@ -1500,7 +1578,7 @@ __device__ __forceinline__ uint32_t slow_group_ticks_c(const Tick4ArgsT<Off> &A,
     const uint64_t adv = a.s.committed[i] - c0;
     d.delta[i] = (uint8_t)(adv > 255u ? 255u : adv);
   }
-  compact_group(a0.s, A.c, A.base_index, A.base_term, a0.gs, (uint32_t)R, i);
+  compact_group(a0.s, A.c, A.base_index, A.base_term, a0.gs, (uint32_t)R, i, tick0 + A.nticks, a0.election_tick, a0.heartbeat_tick);
   return ev;
 }
 
@@ -1511,17 +1589,18 @@ __device__ __forceinline__ uint32_t slow_group_ticks_c(const Tick4ArgsT<Off> &A,
 template <int R>
 struct CStepResult {
   CGroup<R> g;
-  uint32_t out, adv, dirty, slow;
+  uint32_t out, adv, dirty, slow, hb;
 };
 template <int R>
 __device__ __noinline__ CStepResult<R> compact_step_cold(CGroup<R> g, uint32_t flag, uint32_t w0123, uint32_t w4567, uint32_t nprop,
-                                                         uint32_t gate, uint32_t et, uint32_t ht) {
+                                                         uint32_t gate, uint32_t et, uint32_t ht, uint32_t hb) {
   uint32_t wb[R > 1 ? R - 1 : 1];
 #pragma unroll
   for (int j = 0; j < (R > 1 ? R - 1 : 1); ++j) wb[j] = ((j < 4 ? w0123 : w4567) >> (8 * (j & 3))) & 0xFFu;  // the group's R-1 bytes, packed
   CStepResult<R> r;
-  r.slow = compact_step<R, CompactOff>(g, flag, wb, nprop, gate, et, ht, r.out, r.adv, r.dirty) ? 1u : 0u;
+  r.slow = compact_step<R, CompactOff>(g, flag, wb, nprop, gate, et, ht, r.out, r.adv, r.dirty, &hb) ? 1u : 0u;
   r.g = g;
+  r.hb = hb;
   return r;
 }
 #endif
@@ -1615,6 +1694,18 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
   const bool gather = a.world > 1;
   u32x4 iblo{};
   if (gather) iblo = ld_v4u32_p(A.c.iblo + i, pol_keep);
+  uint32_t settled = 0;  // bit k: group k is a settled leader (compact_settled), for the whole launch
+#pragma unroll
+  for (int k = 0; k < 4; ++k) settled |= compact_settled(flag[k], g[k].meta) ? 1u << k : 0u;
+  // The compact leaders' heartbeatElapsed, one byte per group, counted in registers from the phases in c.clk.  With
+  // HeartbeatTick 1 every tick beats and nothing needs counting.  (The bytes of other groups are never used.)
+  uint32_t hb4 = 0;
+  if (a.heartbeat_tick > 1u) {
+    const u32x4 ck = ld_v4u32_p(A.c.clk + i, pol_keep);
+    const uint64_t tick0 = *a.tick_cur;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) hb4 |= (clk_value((ck.v[k] >> 16) & 0xFFu, tick0, a.heartbeat_tick) & 0xFFu) << (8 * k);
+  }
   uint32_t acc_dirty = 0, ncommit = 0;
   // Frames are loaded TWO ticks ahead of their use (a shard of a many-GPU job has too few warps per SM to hide a load
   // behind other warps: the thread's own next ticks have to cover it), and the per-tick descriptors come from shared
@@ -1662,19 +1753,22 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
       uint32_t o, adv, dirty;
       const uint32_t np = (pb >> (8 * k)) & 0xFFu;
       bool slow = false;
-      if (!compact_hot_step<R, CompactOff>(g[k], flag[k], wk, np, gate.v[k], a.election_tick, a.heartbeat_tick, o, adv, dirty)) {
+      if (!compact_hot_step_clk<R, CompactOff>(g[k], (settled >> k) & 1u, flag[k], wk, np, gate.v[k], a.heartbeat_tick, hb4, 8 * k, o,
+                                               adv, dirty)) {
         uint32_t p0 = 0, p1 = 0;  // the group's bytes, four to a word
 #pragma unroll
         for (int j = 0; j < R - 1; ++j) {
           if (j < 4) p0 |= wk[j] << (8 * j);
           else p1 |= wk[j] << (8 * (j - 4));
         }
-        const CStepResult<R> cr = compact_step_cold<R>(g[k], flag[k], p0, p1, np, gate.v[k], a.election_tick, a.heartbeat_tick);
+        const CStepResult<R> cr = compact_step_cold<R>(g[k], flag[k], p0, p1, np, gate.v[k], a.election_tick, a.heartbeat_tick,
+                                                       (hb4 >> (8 * k)) & 0xFFu);
         g[k] = cr.g;
         o = cr.out;
         adv = cr.adv;
         dirty = cr.dirty;
         slow = cr.slow != 0u;
+        hb4 = (hb4 & ~(0xFFu << (8 * k))) | ((cr.hb & 0xFFu) << (8 * k));
       }
       if (slow) {
         newly |= 1u << k;
@@ -1802,6 +1896,9 @@ __global__ void __launch_bounds__(128, 7) tick_fast1_kernel(const Tick4ArgsT<Com
   const uint32_t gate = (flag & CF_GATE_OPEN) ? 0u : ld_stream_u16_p(A.c.gate + i, pol_keep);
   const bool gather = a.world > 1;
   const uint32_t iblo = gather ? ld_stream_u32_p(A.c.iblo + i, pol_keep) : 0u;
+  const bool settled = compact_settled(flag, g.meta);  // (as in tick_fast4_kernel)
+  uint32_t hb = 0;
+  if (a.heartbeat_tick > 1u) hb = clk_value((ld_stream_u32_p(A.c.clk + i, pol_keep) >> 16) & 0xFFu, *a.tick_cur, a.heartbeat_tick) & 0xFFu;
   constexpr int NW = R > 1 ? R - 1 : 1;
   auto load_frame = [&](uint32_t t, uint32_t (&w)[NW], uint32_t &np) {
     const TickDesc &dd = s_desc[t];
@@ -1830,19 +1927,20 @@ __global__ void __launch_bounds__(128, 7) tick_fast1_kernel(const Tick4ArgsT<Com
     bool newly = false;
     const uint32_t lo_old = iblo + g.commit;
     if (!stopped) {
-      if (!compact_hot_step<R, CompactOff>(g, flag, wb, pb, gate, a.election_tick, a.heartbeat_tick, o, adv, dirty)) {
+      if (!compact_hot_step_clk<R, CompactOff>(g, settled, flag, wb, pb, gate, a.heartbeat_tick, hb, 0, o, adv, dirty)) {
         uint32_t p0 = 0, p1 = 0;
 #pragma unroll
         for (int j = 0; j < R - 1; ++j) {
           if (j < 4) p0 |= wb[j] << (8 * j);
           else p1 |= wb[j] << (8 * (j - 4));
         }
-        const CStepResult<R> cr = compact_step_cold<R>(g, flag, p0, p1, pb, gate, a.election_tick, a.heartbeat_tick);
+        const CStepResult<R> cr = compact_step_cold<R>(g, flag, p0, p1, pb, gate, a.election_tick, a.heartbeat_tick, hb);
         g = cr.g;
         o = cr.out;
         adv = cr.adv;
         dirty = cr.dirty;
         newly = cr.slow != 0u;
+        hb = cr.hb;
       }
       if (newly) {
         o = 0;
@@ -1937,19 +2035,21 @@ __global__ void __launch_bounds__(kTickThreads, (R <= 5 ? 6 : 5)) tick_slow4_ker
   }
 }
 
-// whole-engine passes between the two representations (import / export / a new window base / a mode switch)
+// whole-engine passes between the two representations (import / export / a new window base / a mode switch); `T` is
+// the number of the next tick to run (the host's count at enqueue time: stream order makes it exact)
 __global__ void __launch_bounds__(256) materialise_all_kernel(StateView s, CompactViewT<CompactOff> c, uint64_t *base_index, uint64_t gs, uint64_t G,
-                                                               uint32_t R, int clear_flags) {
+                                                               uint32_t R, int clear_flags, uint64_t T, uint32_t et, uint32_t ht) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= G) return;
-  materialise_group(s, c, base_index, gs, R, i);
+  materialise_group(s, c, base_index, gs, R, i, T, et, ht);
   if (clear_flags) c.flag[i] = 0;
 }
 __global__ void __launch_bounds__(256) compact_all_kernel(StateView s, CompactViewT<CompactOff> c, const uint64_t *base_index,
-                                                           const uint64_t *base_term, uint64_t gs, uint64_t G, uint32_t R) {
+                                                           const uint64_t *base_term, uint64_t gs, uint64_t G, uint32_t R, uint64_t T,
+                                                           uint32_t et, uint32_t ht) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= G) return;
-  compact_group(s, c, base_index, base_term, gs, R, i);
+  compact_group(s, c, base_index, base_term, gs, R, i, T, et, ht);
 }
 #endif  // !MRQ_HOST_EMULATION
 
