@@ -66,10 +66,24 @@ tests/cpp/tick_clock_host_test: $(TICKCLOCK_DEP)
 	$(CXX) -std=c++17 -O1 -I$(CUDA_INC) -pthread -o $@ $(TICKCLOCK_SRC)
 tests/cpp/tick_clock_host_test_san: $(TICKCLOCK_DEP)
 	$(SAN_CXX) -std=c++17 -O0 -fsanitize=address,undefined -fno-sanitize-recover=undefined -I$(CUDA_INC) -pthread -o $@ $(TICKCLOCK_SRC)
+# compact_hot_pair (the quad kernel's two-groups-in-16-bit-lanes hot step) against two scalar hot steps.
+TICKPAIR_DEP := tests/cpp/tick_pair_host_test.cpp tests/cpp/device_on_host.hpp $(HDR)
+tests/cpp/tick_pair_host_test: $(TICKPAIR_DEP)
+	$(CXX) -std=c++17 -O1 -I$(CUDA_INC) -o $@ tests/cpp/tick_pair_host_test.cpp
+tests/cpp/tick_pair_host_test_san: $(TICKPAIR_DEP)
+	$(SAN_CXX) -std=c++17 -O0 -fsanitize=address,undefined -fno-sanitize-recover=undefined -I$(CUDA_INC) -o $@ tests/cpp/tick_pair_host_test.cpp
+# Every case of tick_clock_host_test with the quad kernel's pair structure (it includes tick_clock_host_test.cpp).
+TICKPAIRCLOCK_SRC := tests/cpp/tick_pair_clock_host_test.cpp oracle/raft_oracle.c
+TICKPAIRCLOCK_DEP := $(TICKPAIRCLOCK_SRC) $(TICKCLOCK_DEP)
+tests/cpp/tick_pair_clock_host_test: $(TICKPAIRCLOCK_DEP)
+	$(CXX) -std=c++17 -O1 -I$(CUDA_INC) -pthread -o $@ $(TICKPAIRCLOCK_SRC)
+tests/cpp/tick_pair_clock_host_test_san: $(TICKPAIRCLOCK_DEP)
+	$(SAN_CXX) -std=c++17 -O0 -fsanitize=address,undefined -fno-sanitize-recover=undefined -I$(CUDA_INC) -pthread -o $@ $(TICKPAIRCLOCK_SRC)
 
 clean:
 	rm -f $(LIB) $(HOSTLIB) $(CPPTEST) tests/cpp/raftpipe_test_asan tests/cpp/raftpipe_test_tsan build_ptxas.log \
 	  tests/cpp/tick_host_test tests/cpp/tick_host_test_san tests/cpp/tick_host16_test tests/cpp/tick_host16_test_san \
-	  tests/cpp/tick_clock_host_test tests/cpp/tick_clock_host_test_san
+	  tests/cpp/tick_clock_host_test tests/cpp/tick_clock_host_test_san tests/cpp/tick_pair_host_test tests/cpp/tick_pair_host_test_san \
+	  tests/cpp/tick_pair_clock_host_test tests/cpp/tick_pair_clock_host_test_san
 	$(MAKE) -C oracle clean
 .PHONY: all oracle clean san_cxx

@@ -201,6 +201,31 @@ inline uint32_t ld_stream_u32_p(const uint32_t *p, uint64_t) { return *p; }
 inline uint64_t ld_state_p(const uint64_t *p, uint64_t) { return *p; }
 inline void st_state_p(uint64_t *p, uint64_t v, uint64_t) { *p = v; }
 inline void st_state_u32_p(uint32_t *p, uint32_t v, uint64_t) { *p = v; }
+// The byte permute and the 16x2 lane instructions of compact_hot_pair, from the CUDA math API's definitions: per
+// halfword, unsigned, the add wrapping mod 2^16.  (PRMT in its default mode: selector nibble n picks byte (s >> 4n) & 7
+// of {b, a}.)
+inline uint32_t __byte_perm(uint32_t a, uint32_t b, uint32_t s) {
+  const uint64_t x = ((uint64_t)b << 32) | a;
+  uint32_t r = 0;
+  for (int n = 0; n < 4; ++n) r |= (uint32_t)((x >> (8 * ((s >> (4 * n)) & 7u))) & 0xFFu) << (8 * n);
+  return r;
+}
+inline uint32_t lane16_of(uint32_t v, int s) { return (v >> s) & 0xFFFFu; }
+inline uint32_t lanes16_pack(uint32_t lo, uint32_t hi) { return (lo & 0xFFFFu) | ((hi & 0xFFFFu) << 16); }
+inline uint32_t __vminu2(uint32_t a, uint32_t b) {
+  const uint32_t l0 = lane16_of(a, 0) < lane16_of(b, 0) ? lane16_of(a, 0) : lane16_of(b, 0);
+  const uint32_t l1 = lane16_of(a, 16) < lane16_of(b, 16) ? lane16_of(a, 16) : lane16_of(b, 16);
+  return lanes16_pack(l0, l1);
+}
+inline uint32_t __vmaxu2(uint32_t a, uint32_t b) {
+  const uint32_t l0 = lane16_of(a, 0) > lane16_of(b, 0) ? lane16_of(a, 0) : lane16_of(b, 0);
+  const uint32_t l1 = lane16_of(a, 16) > lane16_of(b, 16) ? lane16_of(a, 16) : lane16_of(b, 16);
+  return lanes16_pack(l0, l1);
+}
+inline uint32_t __vimax3_u16x2(uint32_t a, uint32_t b, uint32_t c) { return __vmaxu2(__vmaxu2(a, b), c); }
+inline uint32_t __viaddmax_u16x2(uint32_t a, uint32_t b, uint32_t c) {  // max(a + b, c) per lane, the sum wrapping
+  return __vmaxu2(lanes16_pack(lane16_of(a, 0) + lane16_of(b, 0), lane16_of(a, 16) + lane16_of(b, 16)), c);
+}
 #endif
 
 // ---- q-th largest of R values held in registers (a15: mis[q()-1] after a descending sort) -------
@@ -1332,25 +1357,139 @@ __device__ __forceinline__ bool compact_hot_step(CGroup<R> &g, const uint32_t fl
   return true;
 }
 
+// A compact leader's tickHeartbeat on the clock: its heartbeatElapsed is the byte at bit `shift` of `hbw`, a countdown
+// kept in registers (only looked at when HeartbeatTick > 1).  Returns the out bit.
+__device__ __forceinline__ uint32_t clk_heartbeat(const uint32_t ht, uint32_t &hbw, const uint32_t shift) {
+  if (ht <= 1u) return MRQ_OUT_BCAST_HEARTBEAT;  // HeartbeatTick 1 (reference raft.go:155; launch-uniform): every tick beats
+  uint32_t hb = ((hbw >> shift) & 0xFFu) + 1u;
+  hb = hb >= ht ? 0u : hb;
+  hbw = (hbw & ~(0xFFu << shift)) | (hb << shift);
+  return hb == 0u ? MRQ_OUT_BCAST_HEARTBEAT : 0u;
+}
+
 // The hot step with clock-relative timers (c.clk): `settled` is compact_settled() of the group, evaluated once per
-// launch, and its heartbeatElapsed is the byte at bit `shift` of `hbw`, a countdown kept in registers (only looked at
-// when HeartbeatTick > 1).  The election timer needs no work at all, and neither meta nor c.clk changes.
+// launch, and its heartbeatElapsed is the byte at bit `shift` of `hbw` (clk_heartbeat).  The election timer needs no
+// work at all, and neither meta nor c.clk changes.
 template <int R, typename Off>
 __device__ __forceinline__ bool compact_hot_step_clk(CGroup<R> &g, const bool settled, const uint32_t flag,
                                                      const uint32_t (&wb)[R > 1 ? R - 1 : 1], const uint32_t nprop, const uint32_t gate,
                                                      const uint32_t ht, uint32_t &hbw, const uint32_t shift, uint32_t &out, uint32_t &adv,
                                                      uint32_t &dirty) {
   if (!compact_hot_log<R, Off>(g, settled, flag, wb, nprop, gate, out, adv, dirty)) return false;
-  if (ht <= 1u) {  // HeartbeatTick 1 (reference raft.go:155; launch-uniform): every tick beats
-    out |= MRQ_OUT_BCAST_HEARTBEAT;
-  } else {
-    uint32_t hb = ((hbw >> shift) & 0xFFu) + 1u;
-    hb = hb >= ht ? 0u : hb;
-    if (hb == 0u) out |= MRQ_OUT_BCAST_HEARTBEAT;
-    hbw = (hbw & ~(0xFFu << shift)) | (hb << shift);
-  }
+  out |= clk_heartbeat(ht, hbw, shift);
   return true;
 }
+
+// The (Q-1)-th largest of the R-1 remote rows per lane (Q = R/2 + 1), and their maximum in `vmax`.
+template <int R>
+__device__ __forceinline__ uint32_t pair_kth_largest(const uint32_t (&v)[R > 1 ? R - 1 : 1], uint32_t &vmax) {
+  constexpr int N = R - 1, K = R / 2;  // the K-th largest of N
+  if constexpr (N <= 0) {
+    vmax = 0;
+    return 0;
+  } else if constexpr (N == 1) {
+    vmax = v[0];
+    return v[0];
+  } else if constexpr (N == 2) {  // K = 1
+    vmax = __vmaxu2(v[0], v[1]);
+    return vmax;
+  } else if constexpr (N == 3) {  // K = 2: the median of 3
+    const uint32_t lo = __vminu2(v[0], v[1]), hi = __vmaxu2(v[0], v[1]);
+    vmax = __vmaxu2(hi, v[2]);
+    return __vmaxu2(lo, __vminu2(hi, v[2]));
+  } else if constexpr (N == 4) {  // K = 2: the second largest of 4
+    const uint32_t lo01 = __vminu2(v[0], v[1]), hi01 = __vmaxu2(v[0], v[1]);
+    const uint32_t lo23 = __vminu2(v[2], v[3]), hi23 = __vmaxu2(v[2], v[3]);
+    vmax = __vmaxu2(hi01, hi23);
+    return __vimax3_u16x2(__vminu2(hi01, hi23), lo01, lo23);
+  } else {  // partial selection: K passes of bubbling maxima to the front
+    uint32_t w[N];
+#pragma unroll
+    for (int i = 0; i < N; ++i) w[i] = v[i];
+#pragma unroll
+    for (int p = 0; p < K; ++p) {
+#pragma unroll
+      for (int i = N - 1; i > p; --i) {
+        const uint32_t a = w[i - 1], b = w[i];
+        w[i - 1] = __vmaxu2(a, b);
+        w[i] = __vminu2(a, b);
+      }
+    }
+    vmax = w[0];
+    return w[K - 1];
+  }
+}
+
+// ---- the hot step of TWO groups at once, in the 16-bit lanes of Hopper's 16x2 integer instructions ----------------
+// The quad kernel keeps each 16-bit offset column as two u32 words, the pair words: word 0 holds groups 0 (low half)
+// and 1 (high half) of the quad, word 1 groups 2 and 3 — exactly as the column lies in memory.  compact_hot_pair runs
+// compact_hot_log for both groups of one pair on those words, one VIMNMX / VIADDMNMX .U16x2 per step where the scalar
+// step needs one instruction per group, and gives each lane exactly what the scalar step gives its group.  It applies
+// only where that is cheap to make exact; otherwise it returns false with nothing changed, and the caller runs the
+// scalar steps.  The caller vouches, once per launch, that both groups are settled leaders (compact_settled) still on
+// the fast path.  Per tick it declines unless, in both lanes:
+//   - every frame byte is "no message" or an ack (kind 0 or 1: no kind 2 or 3);
+//   - every Match after the acks is <= lastIndex: for a settled (not strict) leader every stored Match is <= lastIndex,
+//     so this is the scalar step's "no ack beyond lastIndex";
+//   - lastIndex <= span - 255 and win <= 0xFFBF: no lane sum can wrap (win + 63 <= 0xFFFE, lastIndex + 255 <= span),
+//     and the scalar "lastIndex + nprop <= span" holds.  A group is that close to the top only every ~43k ticks, for a
+//     few hundred entries; the scalar step then makes the exact re-base decision.
+// The commit is mci = max(commit, Q-th largest Match), never commit + q: an order statistic commutes with max(., commit),
+// so this is the scalar max(m, commit) - commit network, and mci <= lastIndex by construction.  Since the new lastIndex
+// is the largest row, the Q-th largest of R rows is the (Q-1)-th largest of the R-1 remote rows.  As in the scalar step,
+// a lane whose Match and lastIndex did not move keeps its commit (after an import commit may sit below the quorum).
+// `gate2`: c.gate in the lanes whose commit gate is still closed (CF_GATE_OPEN clear), 0 in the others; such a lane
+// commits only an index >= its gate, as maybeCommit's term check does in the scalar step.
+// Outputs per lane: `q2` the commit advance, `out2` MRQ_OUT_BCAST_APPEND / MRQ_OUT_COMMIT_ADVANCED (the heartbeat is
+// the caller's), and `dirty` the pair's CD_MATCH0 / CD_COMMIT / CD_WIN.  `wq`: the quad's frame words (byte k = group k),
+// `pq`: its proposal bytes, `hi`: 0 for groups 0/1, 1 for groups 2/3.
+template <int R>
+__device__ __forceinline__ bool compact_hot_pair(uint32_t &commit2, uint32_t &win2, uint32_t (&m2)[R], const uint32_t gate2,
+                                                 const uint32_t (&wq)[R > 1 ? R - 1 : 1], const uint32_t pq, const int hi, uint32_t &q2,
+                                                 uint32_t &out2, uint32_t &dirty) {
+  constexpr uint32_t kLo = 0x00010001u;  // 1 in each lane
+  const uint32_t span = compact_span<uint16_t>();
+  if (span < 0xFFu) return false;  // (only a host test's tiny span)
+  const uint32_t li_cap = (span - 0xFFu) * kLo, win_cap = 0xFFBFu * kLo;
+  const uint32_t sel = hi ? 0x4342u : 0x4140u;  // the pair's two bytes into the low byte of each lane
+  const uint32_t li = m2[R - 1];
+  if (__vmaxu2(li, li_cap) != li_cap || __vmaxu2(win2, win_cap) != win_cap) return false;
+  uint32_t nm[R > 1 ? R - 1 : 1], kinds = 0, moved = 0, mn = 0x01000100u;
+#pragma unroll
+  for (int j = 0; j < R - 1; ++j) {
+    const uint32_t b = __byte_perm(wq[j], 0u, sel);  // a frame byte per lane: payload << 2 | kind
+    kinds |= b;
+    const uint32_t ack = (b & kLo) * 0xFFFFu;            // 0xFFFF in a lane with an ack
+    const uint32_t pay = (b >> 2) & ack & 0x003F003Fu;   // the ack's payload, 0 elsewhere
+    nm[j] = __viaddmax_u16x2(win2 & ack, pay, m2[j]);    // Progress.maybeUpdate(win + pay)
+    moved |= nm[j] ^ m2[j];
+    mn = __vminu2(mn, (b & ack) | (~ack & 0x01000100u));  // min ack byte; 0x100 (payload 64): no ack
+  }
+  if ((kinds & 0x00020002u) != 0u) return false;  // a heartbeat, a response, an escape: not the hot case
+  uint32_t nmax = 0;
+  const uint32_t kth = pair_kth_largest<R>(nm, nmax);
+  if (R > 1 && __vmaxu2(nmax, li) != li) return false;  // an ack beyond lastIndex
+  const uint32_t np = __byte_perm(pq, 0u, sel);
+  const uint32_t nli = li + np;  // (no lane carries: li <= span - 255)
+  moved |= np;
+  const uint32_t mmask = __vminu2(moved, kLo) * 0xFFFFu;  // 0xFFFF in a lane whose Match or lastIndex moved
+  const uint32_t mc = __vmaxu2(commit2, (R > 1 ? kth : nli) & mmask);
+  const uint32_t shut = __vminu2(__vmaxu2(gate2, mc) ^ mc, kLo) * 0xFFFFu;  // 0xFFFF in a lane whose gate is above mc
+  const uint32_t mci = (mc & ~shut) | (commit2 & shut);
+  q2 = mci - commit2;  // (mci >= commit in both lanes: no lane borrows)
+  // the window slides by min_ack - 16 when 16 < min_ack < 64: (min_ack & 63) maps the "no ack" 64 to 0
+  const uint32_t slide16 = __vmaxu2((mn >> 2) & 0x003F003Fu, 0x00100010u);  // 16 + the slide
+  const uint32_t nwin = win2 + slide16 - 0x00100010u;
+  out2 = __vminu2(np | q2, kLo) * MRQ_OUT_BCAST_APPEND + __vminu2(q2, kLo) * MRQ_OUT_COMMIT_ADVANCED;
+  dirty = (moved != 0u ? CD_MATCH0 : 0u) | (q2 != 0u ? CD_COMMIT : 0u) | (nwin != win2 ? CD_WIN : 0u);
+#pragma unroll
+  for (int j = 0; j < R - 1; ++j) m2[j] = nm[j];
+  m2[R - 1] = nli;
+  commit2 = mci;
+  win2 = nwin;
+  return true;
+}
+
 
 // One tick of one group on compact state, every case the compact form can express.  Returns true (and leaves `g`
 // untouched) when the group needs the general path.  `wb[j]`: the frame's byte of row j, `nprop`: the proposal byte,
@@ -1628,16 +1767,22 @@ __device__ __forceinline__ void ld_v2u64_p(const uint64_t *p, uint64_t pol, uint
 __device__ __forceinline__ void st_v2u64_p(uint64_t *p, uint64_t a, uint64_t b, uint64_t pol) {
   asm volatile("st.global.L1::no_allocate.L2::cache_hint.v2.u64 [%0], {%1, %2}, %3;" ::"l"(p), "l"(a), "l"(b), "l"(pol) : "memory");
 }
-// The 16-bit offset columns: a quad is one 64-bit access, widened to u32 at the load and narrowed at the store
-__device__ __forceinline__ u32x4 ld_v4u16_p(const uint16_t *p, uint64_t pol) {
-  uint32_t a, b;
+// The 16-bit offset columns: a quad is one 64-bit access, two pair words (compact_hot_pair) as they lie in memory
+__device__ __forceinline__ void ld_pairs_p(const uint16_t *p, uint64_t pol, uint32_t &a, uint32_t &b) {
   asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v2.u32 {%0, %1}, [%2], %3;" : "=r"(a), "=r"(b) : "l"(p), "l"(pol));
+}
+__device__ __forceinline__ void st_pairs_p(uint16_t *p, uint32_t a, uint32_t b, uint64_t pol) {
+  asm volatile("st.global.L1::no_allocate.L2::cache_hint.v2.u32 [%0], {%1, %2}, %3;" ::"l"(p), "r"(a), "r"(b), "l"(pol) : "memory");
+}
+__device__ __forceinline__ u32x4 ld_v4u16_p(const uint16_t *p, uint64_t pol) {  // (widened to one u32 per group)
+  uint32_t a, b;
+  ld_pairs_p(p, pol, a, b);
   return u32x4{{__byte_perm(a, 0u, 0x4410), __byte_perm(a, 0u, 0x4432), __byte_perm(b, 0u, 0x4410), __byte_perm(b, 0u, 0x4432)}};
 }
-__device__ __forceinline__ void st_v4u16_p(uint16_t *p, const u32x4 &r, uint64_t pol) {
-  asm volatile("st.global.L1::no_allocate.L2::cache_hint.v2.u32 [%0], {%1, %2}, %3;" ::"l"(p), "r"(__byte_perm(r.v[0], r.v[1], 0x5410)),
-               "r"(__byte_perm(r.v[2], r.v[3], 0x5410)), "l"(pol)
-               : "memory");
+// group k of a quad held as pair words: get / set its 16-bit lane
+__device__ __forceinline__ uint32_t lane16(const uint32_t (&w)[2], int k) { return (w[k >> 1] >> (16 * (k & 1))) & 0xFFFFu; }
+__device__ __forceinline__ void set_lane16(uint32_t (&w)[2], int k, uint32_t v) {
+  w[k >> 1] = __byte_perm(w[k >> 1], v, (k & 1) ? 0x5410u : 0x3254u);
 }
 __device__ __forceinline__ uint32_t ld_stream_u16_p(const uint16_t *p, uint64_t pol) {
   uint32_t v;
@@ -1665,38 +1810,37 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
   pdl_wait();
   if (blockIdx.x == 0 && threadIdx.x == 0) *a.tick_next = *a.tick_cur + A.nticks;
   // ---- the quad's state: one wave of independent 128-bit loads ---------------------------------------------------
-  CGroup<R> g[4];
-  uint32_t flag[4];
+  // The offsets stay packed as pair words (compact_hot_pair): cm2[p], wn2[p] and m2[p][r] hold groups 2p and 2p + 1.
+  uint64_t meta[4];
+  uint32_t flag[4], cm2[2], wn2[2], m2[2][R];
   {
     const uint32_t fw = ld_stream_u32_p(reinterpret_cast<const uint32_t *>(A.c.flag + i), pol_keep);
-    ld_v2u64_p(a.s.meta + i, pol_keep, g[0].meta, g[1].meta);
-    ld_v2u64_p(a.s.meta + i + 2, pol_keep, g[2].meta, g[3].meta);
-    const u32x4 cm = ld_v4u16_p(A.c.commit + i, pol_keep);
-    const u32x4 wn = ld_v4u16_p(A.c.win + i, pol_keep);
-    u32x4 mv[R];
+    ld_v2u64_p(a.s.meta + i, pol_keep, meta[0], meta[1]);
+    ld_v2u64_p(a.s.meta + i + 2, pol_keep, meta[2], meta[3]);
+    ld_pairs_p(A.c.commit + i, pol_keep, cm2[0], cm2[1]);
+    ld_pairs_p(A.c.win + i, pol_keep, wn2[0], wn2[1]);
 #pragma unroll
-    for (int r = 0; r < R; ++r) mv[r] = ld_v4u16_p(A.c.match + (uint64_t)r * a.gs + i, pol_keep);
+    for (int r = 0; r < R; ++r) ld_pairs_p(A.c.match + (uint64_t)r * a.gs + i, pol_keep, m2[0][r], m2[1][r]);
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      flag[k] = (fw >> (8 * k)) & 0xFFu;
-      g[k].commit = cm.v[k];
-      g[k].win = wn.v[k];
-#pragma unroll
-      for (int r = 0; r < R; ++r) g[k].m[r] = mv[r].v[k];
-    }
+    for (int k = 0; k < 4; ++k) flag[k] = (fw >> (8 * k)) & 0xFFu;
   }
   uint32_t stopped = 0;  // bit k: group k is not this kernel's (padding, or handed to the general path at an earlier tick)
 #pragma unroll
   for (int k = 0; k < 4; ++k)
     if (!active || i0 + k >= a.G) stopped |= 1u << k;
-  u32x4 gate{};  // only the few groups whose commit gate is still closed look at it
-  if (((flag[0] & flag[1] & flag[2] & flag[3]) & CF_GATE_OPEN) == 0u) gate = ld_v4u16_p(A.c.gate + i, pol_keep);
+  uint32_t gt2[2] = {0u, 0u};  // c.gate in the lanes of the few groups whose commit gate is still closed, else 0
+  if (((flag[0] & flag[1] & flag[2] & flag[3]) & CF_GATE_OPEN) == 0u) {
+    ld_pairs_p(A.c.gate + i, pol_keep, gt2[0], gt2[1]);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (flag[k] & CF_GATE_OPEN) set_lane16(gt2, k, 0u);
+  }
   const bool gather = a.world > 1;
   u32x4 iblo{};
   if (gather) iblo = ld_v4u32_p(A.c.iblo + i, pol_keep);
   uint32_t settled = 0;  // bit k: group k is a settled leader (compact_settled), for the whole launch
 #pragma unroll
-  for (int k = 0; k < 4; ++k) settled |= compact_settled(flag[k], g[k].meta) ? 1u << k : 0u;
+  for (int k = 0; k < 4; ++k) settled |= compact_settled(flag[k], meta[k]) ? 1u << k : 0u;
   // The compact leaders' heartbeatElapsed, one byte per group, counted in registers from the phases in c.clk.  With
   // HeartbeatTick 1 every tick beats and nothing needs counting.  (The bytes of other groups are never used.)
   uint32_t hb4 = 0;
@@ -1706,7 +1850,7 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
 #pragma unroll
     for (int k = 0; k < 4; ++k) hb4 |= (clk_value((ck.v[k] >> 16) & 0xFFu, tick0, a.heartbeat_tick) & 0xFFu) << (8 * k);
   }
-  uint32_t acc_dirty = 0, ncommit = 0;
+  uint32_t acc_dirty = 0, ncommit = 0, ncommit2 = 0;  // ncommit2: the pair steps' count, per lane
   // Frames are loaded TWO ticks ahead of their use (a shard of a many-GPU job has too few warps per SM to hide a load
   // behind other warps: the thread's own next ticks have to cover it), and the per-tick descriptors come from shared
   // memory, so that a frame load never waits for a descriptor load first.
@@ -1738,47 +1882,74 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
     if (t + 2 < A.nticks) load_frame(t + 2, wb2, pb2);
     const TickDesc &d = s_desc[t];
     u32x4 outw{};
-    uint32_t dw = 0, newly = 0, tdirty = 0;
+    uint32_t adv2[2] = {0u, 0u}, newly = 0, tdirty = 0;  // adv2: the commit advance bytes, in the pair words' lanes
     u32x4 lo_old{};
     if (gather) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) lo_old.v[k] = iblo.v[k] + g[k].commit;
+      for (int k = 0; k < 4; ++k) lo_old.v[k] = iblo.v[k] + lane16(cm2, k);
     }
+    const uint32_t pair_ok = settled & ~stopped;
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if (stopped & (1u << k)) continue;
-      uint32_t wk[R > 1 ? R - 1 : 1];
+    for (int p = 0; p < 2; ++p) {
+      uint32_t q2, o2, pd;
+      if (((pair_ok >> (2 * p)) & 3u) == 3u && compact_hot_pair<R>(cm2[p], wn2[p], m2[p], gt2[p], wb, pb, p, q2, o2, pd)) {
 #pragma unroll
-      for (int j = 0; j < (R > 1 ? R - 1 : 1); ++j) wk[j] = (wb[j] >> (8 * k)) & 0xFFu;
-      uint32_t o, adv, dirty;
-      const uint32_t np = (pb >> (8 * k)) & 0xFFu;
-      bool slow = false;
-      if (!compact_hot_step_clk<R, CompactOff>(g[k], (settled >> k) & 1u, flag[k], wk, np, gate.v[k], a.heartbeat_tick, hb4, 8 * k, o,
-                                               adv, dirty)) {
-        uint32_t p0 = 0, p1 = 0;  // the group's bytes, four to a word
+        for (int h = 0; h < 2; ++h) outw.v[2 * p + h] = ((o2 >> (16 * h)) & 0xFFFFu) | clk_heartbeat(a.heartbeat_tick, hb4, 8 * (2 * p + h));
+        adv2[p] = __vminu2(q2, 0x00FF00FFu);
+        ncommit2 += __vminu2(q2, 0x00010001u);
+        tdirty |= pd;
+        continue;
+      }
+      // the pair declined: the scalar steps, one group at a time, unpacked here and repacked after
 #pragma unroll
-        for (int j = 0; j < R - 1; ++j) {
-          if (j < 4) p0 |= wk[j] << (8 * j);
-          else p1 |= wk[j] << (8 * (j - 4));
+      for (int h = 0; h < 2; ++h) {
+        const int k = 2 * p + h;
+        if (stopped & (1u << k)) continue;
+        CGroup<R> g;
+        g.meta = meta[k];
+        g.commit = lane16(cm2, k);
+        g.win = lane16(wn2, k);
+#pragma unroll
+        for (int r = 0; r < R; ++r) g.m[r] = (m2[p][r] >> (16 * h)) & 0xFFFFu;
+        uint32_t wk[R > 1 ? R - 1 : 1];
+#pragma unroll
+        for (int j = 0; j < (R > 1 ? R - 1 : 1); ++j) wk[j] = (wb[j] >> (8 * k)) & 0xFFu;
+        uint32_t o, adv, dirty;
+        const uint32_t np = (pb >> (8 * k)) & 0xFFu;
+        bool slow = false;
+        if (!compact_hot_step_clk<R, CompactOff>(g, (settled >> k) & 1u, flag[k], wk, np, lane16(gt2, k), a.heartbeat_tick, hb4, 8 * k, o, adv,
+                                                 dirty)) {
+          uint32_t p0 = 0, p1 = 0;  // the group's bytes, four to a word
+#pragma unroll
+          for (int j = 0; j < R - 1; ++j) {
+            if (j < 4) p0 |= wk[j] << (8 * j);
+            else p1 |= wk[j] << (8 * (j - 4));
+          }
+          const CStepResult<R> cr = compact_step_cold<R>(g, flag[k], p0, p1, np, lane16(gt2, k), a.election_tick, a.heartbeat_tick,
+                                                         (hb4 >> (8 * k)) & 0xFFu);
+          g = cr.g;
+          o = cr.out;
+          adv = cr.adv;
+          dirty = cr.dirty;
+          slow = cr.slow != 0u;
+          hb4 = (hb4 & ~(0xFFu << (8 * k))) | ((cr.hb & 0xFFu) << (8 * k));
         }
-        const CStepResult<R> cr = compact_step_cold<R>(g[k], flag[k], p0, p1, np, gate.v[k], a.election_tick, a.heartbeat_tick,
-                                                       (hb4 >> (8 * k)) & 0xFFu);
-        g[k] = cr.g;
-        o = cr.out;
-        adv = cr.adv;
-        dirty = cr.dirty;
-        slow = cr.slow != 0u;
-        hb4 = (hb4 & ~(0xFFu << (8 * k))) | ((cr.hb & 0xFFu) << (8 * k));
-      }
-      if (slow) {
-        newly |= 1u << k;
-      } else {
-        outw.v[k] = o;
-        dw |= (adv > 255u ? 255u : adv) << (8 * k);
-        tdirty |= dirty;
-        ncommit += adv != 0u;
+        meta[k] = g.meta;
+        set_lane16(cm2, k, g.commit);
+        set_lane16(wn2, k, g.win);
+#pragma unroll
+        for (int r = 0; r < R; ++r) m2[p][r] = __byte_perm(m2[p][r], g.m[r], h ? 0x5410u : 0x3254u);
+        if (slow) {
+          newly |= 1u << k;
+        } else {
+          outw.v[k] = o;
+          adv2[p] |= (adv > 255u ? 255u : adv) << (16 * h);
+          tdirty |= dirty;
+          ncommit += adv != 0u;
+        }
       }
     }
+    const uint32_t dw = __byte_perm(adv2[0], adv2[1], 0x6420);
     if (__any_sync(0xFFFFFFFFu, newly != 0u)) {  // hand those groups (from this tick on) to the general kernel
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
@@ -1805,7 +1976,7 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
         u32x4 lo;
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          lo.v[k] = iblo.v[k] + g[k].commit;
+          lo.v[k] = iblo.v[k] + lane16(cm2, k);
           lo4 |= (lo.v[k] & 0xFFu) << (8 * k);
           carry = carry || ((lo.v[k] ^ lo_old.v[k]) >> 8) != 0u;  // anything above the low byte moved (a wrap of the
         }                                                         // low word changes bits 8..31 too)
@@ -1825,7 +1996,7 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
 #pragma unroll
           for (int k = 0; k < 4; ++k)
             if (!(stopped & (1u << k)) && (a.gather_prime || ((lo.v[k] ^ lo_old.v[k]) >> 8) != 0u)) {
-              const uint64_t full = A.c.ibase[i + k] + g[k].commit;
+              const uint64_t full = A.c.ibase[i + k] + lane16(cm2, k);
 #pragma unroll 1
               for (uint32_t p = 0; p < a.world; ++p) a.peer_full[p][at + k] = full;
             }
@@ -1838,15 +2009,14 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
       uint32_t wd = __reduce_or_sync(0xFFFFFFFFu, A.write_through ? tdirty : acc_dirty);
       if (active) {  // (a quad whose groups all left the fast path still owes the columns its earlier ticks changed)
         if (wd & CD_META) {
-          st_v2u64_p(a.s.meta + i, g[0].meta, g[1].meta, pol_keep);
-          st_v2u64_p(a.s.meta + i + 2, g[2].meta, g[3].meta, pol_keep);
+          st_v2u64_p(a.s.meta + i, meta[0], meta[1], pol_keep);
+          st_v2u64_p(a.s.meta + i + 2, meta[2], meta[3], pol_keep);
         }
-        if (wd & CD_COMMIT) st_v4u16_p(A.c.commit + i, u32x4{{g[0].commit, g[1].commit, g[2].commit, g[3].commit}}, pol_keep);
-        if (wd & CD_WIN) st_v4u16_p(A.c.win + i, u32x4{{g[0].win, g[1].win, g[2].win, g[3].win}}, pol_keep);
+        if (wd & CD_COMMIT) st_pairs_p(A.c.commit + i, cm2[0], cm2[1], pol_keep);
+        if (wd & CD_WIN) st_pairs_p(A.c.win + i, wn2[0], wn2[1], pol_keep);
         if (wd & CD_MATCH_ANY) {
 #pragma unroll
-          for (int r = 0; r < R; ++r)
-            st_v4u16_p(A.c.match + (uint64_t)r * a.gs + i, u32x4{{g[0].m[r], g[1].m[r], g[2].m[r], g[3].m[r]}}, pol_keep);
+          for (int r = 0; r < R; ++r) st_pairs_p(A.c.match + (uint64_t)r * a.gs + i, m2[0][r], m2[1][r], pol_keep);
         }
       }
     }
@@ -1859,7 +2029,7 @@ __global__ void __launch_bounds__(THREADS, (R <= 5 ? MRQ_T4_THREADS_PER_SM : 384
     pb1 = pb2;
   }
   // "commit advanced" events: one warp-reduced atomic
-  const unsigned tot = __reduce_add_sync(0xFFFFFFFFu, ncommit);
+  const unsigned tot = __reduce_add_sync(0xFFFFFFFFu, ncommit + (ncommit2 & 0xFFFFu) + (ncommit2 >> 16));
   if (tot != 0 && (threadIdx.x & 31u) == 0)
     atomicAdd(&a.ctr[blockIdx.x & (kCtrShards - 1)].commits_advanced, (unsigned long long)tot);
 }
