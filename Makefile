@@ -80,10 +80,20 @@ tests/cpp/tick_pair_clock_host_test: $(TICKPAIRCLOCK_DEP)
 tests/cpp/tick_pair_clock_host_test_san: $(TICKPAIRCLOCK_DEP)
 	$(SAN_CXX) -std=c++17 -O0 -fsanitize=address,undefined -fno-sanitize-recover=undefined -I$(CUDA_INC) -pthread -o $@ $(TICKPAIRCLOCK_SRC)
 
+# The change feed: the general tick's records against the diff of consecutive oracle exports, and the fast functions
+# leaving term / vote / role / lead alone (it includes tick_host_test.cpp for the harness).
+FEEDHOST_SRC := tests/cpp/change_feed_host_test.cpp oracle/raft_oracle.c
+FEEDHOST_DEP := $(FEEDHOST_SRC) $(TICKHOST_DEP)
+tests/cpp/change_feed_host_test: $(FEEDHOST_DEP)
+	$(CXX) -std=c++17 -O1 -I$(CUDA_INC) -pthread -o $@ $(FEEDHOST_SRC)
+tests/cpp/change_feed_host_test_san: $(FEEDHOST_DEP)
+	$(SAN_CXX) -std=c++17 -O0 -fsanitize=address,undefined -fno-sanitize-recover=undefined -I$(CUDA_INC) -pthread -o $@ $(FEEDHOST_SRC)
+
 clean:
 	rm -f $(LIB) $(HOSTLIB) $(CPPTEST) tests/cpp/raftpipe_test_asan tests/cpp/raftpipe_test_tsan build_ptxas.log \
 	  tests/cpp/tick_host_test tests/cpp/tick_host_test_san tests/cpp/tick_host16_test tests/cpp/tick_host16_test_san \
 	  tests/cpp/tick_clock_host_test tests/cpp/tick_clock_host_test_san tests/cpp/tick_pair_host_test tests/cpp/tick_pair_host_test_san \
-	  tests/cpp/tick_pair_clock_host_test tests/cpp/tick_pair_clock_host_test_san
+	  tests/cpp/tick_pair_clock_host_test tests/cpp/tick_pair_clock_host_test_san \
+	  tests/cpp/change_feed_host_test tests/cpp/change_feed_host_test_san
 	$(MAKE) -C oracle clean
 .PHONY: all oracle clean san_cxx

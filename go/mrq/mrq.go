@@ -295,3 +295,53 @@ func (e *Engine) SlotOutputs(slot uint32, out []uint32, delta []byte) error {
 	}
 	return nil
 }
+
+// Change-feed flags: which of HardState {Term, Vote} and SoftState {RaftState, Lead} a tick moved.
+const (
+	ChangeTerm = C.MRQ_CHANGE_TERM
+	ChangeVote = C.MRQ_CHANGE_VOTE
+	ChangeRole = C.MRQ_CHANGE_ROLE
+	ChangeLead = C.MRQ_CHANGE_LEAD
+)
+
+// Change is one change-feed record: group's term, vote, role or lead after tick Tick differ from before it.
+// TermStart is the new leader's empty entry (math.MaxUint64 unless Role == RoleLeader).
+type Change struct {
+	Tick, Term, TermStart uint64
+	Group                 uint32
+	Vote, Role, Lead      uint8
+	What                  uint8 // Change* bits, never 0
+}
+
+// SetChangeCapacity turns the change feed on with room for n records between drains (0 turns it off).
+func (e *Engine) SetChangeCapacity(n uint64) error {
+	if rc := C.mrq_set_change_capacity(e.h, C.uint64_t(n)); rc != 0 {
+		return lastErr(e.h)
+	}
+	return nil
+}
+
+// SyncChanges drains the change feed: every record since the previous drain, sorted by (Tick, Group).  lost > 0
+// means records did not fit the capacity: the list is incomplete and the host must read the state in full.
+func (e *Engine) SyncChanges() (changes []Change, lost uint64, err error) {
+	buf := make([]C.mrq_change, 1024)
+	var n, l C.uint64_t
+	for {
+		rc := C.mrq_sync_changes(e.h, &buf[0], C.uint64_t(len(buf)), &n, &l)
+		if rc == C.MRQ_E_INVAL && uint64(n) > uint64(len(buf)) { // nothing was consumed: retry with room for all
+			buf = make([]C.mrq_change, int(n))
+			continue
+		}
+		if rc != 0 {
+			return nil, 0, lastErr(e.h)
+		}
+		break
+	}
+	changes = make([]Change, int(n))
+	for i := range changes {
+		c := &buf[i]
+		changes[i] = Change{Tick: uint64(c.tick), Term: uint64(c.term), TermStart: uint64(c.term_start), Group: uint32(c.group),
+			Vote: uint8(c.vote), Role: uint8(c.role), Lead: uint8(c.lead), What: uint8(c.what)}
+	}
+	return changes, uint64(l), nil
+}

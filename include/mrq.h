@@ -331,6 +331,30 @@ int mrq_drain_tick_deltas(mrq_engine *e, uint8_t *delta_out_pinned);
 int mrq_sync_slot_outputs(mrq_engine *e, uint32_t slot, uint32_t *out_words, uint8_t *delta_out);
 int mrq_synchronize(mrq_engine *e);
 
+/* ---- change feed: the groups whose HardState {Term, Vote} or SoftState {Lead, RaftState} moved (raft.go:227-235) ----
+ * Recorded by the tick kernels themselves in every tick mode and every way of ticking (mrq_tick, mrq_tick_many,
+ * mrq_tick_idle).  Commit advances are not recorded (they have their own drains); neither are changes the host makes
+ * itself (mrq_import_state, mrq_set_tick_count).  Draining converts no state representation.                      */
+#define MRQ_CHANGE_TERM 0x01u /* HardState.Term moved            */
+#define MRQ_CHANGE_VOTE 0x02u /* HardState.Vote moved            */
+#define MRQ_CHANGE_ROLE 0x04u /* SoftState.RaftState moved       */
+#define MRQ_CHANGE_LEAD 0x08u /* SoftState.Lead moved            */
+typedef struct mrq_change {   /* 32 bytes                        */
+  uint64_t tick;              /* number of the tick that made the change (mrq_tick_count() before it) */
+  uint64_t term;              /* after the tick                   */
+  uint64_t term_start;        /* after the tick; UINT64_MAX unless leader (a new leader's empty entry) */
+  uint32_t group;             /* local group index                */
+  uint8_t vote, role, lead, what; /* after the tick; what = MRQ_CHANGE_* bits, never 0 */
+} mrq_change;
+/* 0 (default) = off.  Otherwise record up to max_records changes between drains.  Blocking; discards pending records. */
+int mrq_set_change_capacity(mrq_engine *e, uint64_t max_records);
+/* Blocking.  Every record since the previous drain, sorted by (tick, group), then reset.  Exactly one record per
+ * (tick, group) whose term, vote, role or lead differs after that tick from before it.  *lost = records that did
+ * not fit the capacity: the list is then incomplete (each returned record is still genuine) and the host must
+ * read state in full.  cap < records pending: MRQ_E_INVAL, nothing consumed, *n_out = entries needed.
+ * Feed off: MRQ_E_STATE. */
+int mrq_sync_changes(mrq_engine *e, mrq_change *out, uint64_t cap, uint64_t *n_out, uint64_t *lost);
+
 /* ---- synthetic vote/append traces, generated on the device (include/mrq_trace.h) -------- */
 struct mrq_trace_params;
 int mrq_gen_trace(mrq_engine *e, uint32_t slot, const struct mrq_trace_params *p, uint64_t tick);

@@ -89,6 +89,16 @@ class TraceParams(C.Structure):
                 ("lagging_pct", C.c_uint32), ("max_prop", C.c_uint32), ("lag_kind", C.c_uint32)]
 
 
+CHANGE_TERM, CHANGE_VOTE, CHANGE_ROLE, CHANGE_LEAD = 0x01, 0x02, 0x04, 0x08
+
+
+class Change(C.Structure):
+    """include/mrq.h `mrq_change`: one change-feed record (32 bytes)."""
+
+    _fields_ = [("tick", C.c_uint64), ("term", C.c_uint64), ("term_start", C.c_uint64), ("group", C.c_uint32),
+                ("vote", C.c_uint8), ("role", C.c_uint8), ("lead", C.c_uint8), ("what", C.c_uint8)]
+
+
 class Counters(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("ticks", "kernel_launches", "campaigns", "elections_won", "step_downs",
                                           "commits_advanced", "votes_granted", "errors")]
@@ -135,6 +145,8 @@ SIGNATURES = {
     "mrq_set_write_through": (C.c_int, [_EP, C.c_int]),
     "mrq_sync_slot_outputs": (C.c_int, [_EP, C.c_uint32, u32p, u8p]),
     "mrq_synchronize": (C.c_int, [_EP]),
+    "mrq_set_change_capacity": (C.c_int, [_EP, C.c_uint64]),
+    "mrq_sync_changes": (C.c_int, [_EP, C.POINTER(Change), C.c_uint64, u64p, u64p]),
     "mrq_gen_trace": (C.c_int, [_EP, C.c_uint32, C.POINTER(TraceParams), C.c_uint64]),
     "mrq_read_inbox": (C.c_int, [_EP, C.c_uint32, C.POINTER(InboxOut)]),
     "mrq_get_counters": (C.c_int, [_EP, C.POINTER(Counters)]),

@@ -140,6 +140,10 @@ struct mrq_engine {
   int write_through = 1;              // multi-tick launches: state columns written after every tick (1) or the last (0)
   uint64_t stage_gen = 0;             // bumps when a staging buffer moves: cached descriptor tables are keyed by it
   std::map<std::string, TickDesc *> desc_tables;
+  // change feed (mrq_set_change_capacity): records the general tick appends, and their count since the last drain
+  mrq_change *changes = nullptr;
+  unsigned long long *change_count = nullptr;
+  uint64_t change_cap = 0;
   std::string err;
 };
 
@@ -304,6 +308,9 @@ void fill_tick_args(mrq_engine *e, TickArgs &a) {
   a.slow_list = e->slow_list;
   a.slow_count = e->slow_count + (e->slow_parity & 1u);
   a.slow_count_next = e->slow_count + ((e->slow_parity + 1u) & 1u);
+  a.changes = e->changes;
+  a.change_count = e->change_count;
+  a.change_cap = e->change_cap;
 }
 
 // n ticks of mode 4 in ONE pair of launches: every slot holds a byte frame (mrq_post_inbox_packed, word_bits 8).
@@ -687,6 +694,8 @@ void mrq_destroy(mrq_engine *e) {
                   e->s.out, e->ctr, e->commit_prev, e->delta, e->gathered, e->scratch, e->pk_base_index, e->pk_base_term, e->slow_list, e->slow_count, e->tickbuf};
   for (auto &kv : e->graphs) cudaGraphExecDestroy(kv.second);
   for (auto &kv : e->desc_tables) cudaFree(kv.second);
+  if (e->changes) cudaFree(e->changes);
+  if (e->change_count) cudaFree(e->change_count);
   {
     void *cp[] = {e->c.flag, e->c.commit, e->c.win, e->c.gate, e->c.iblo, e->c.match, e->c.ibase, e->c.clk, e->slow_list64};
     for (void *p : cp)
@@ -1584,6 +1593,57 @@ int mrq_sync_slot_outputs(mrq_engine *e, uint32_t slot, uint32_t *out_words, uin
   if (e->G && out_words) CK(e, cudaMemcpyAsync(out_words, e->out_slot[slot], e->G * 4, cudaMemcpyDeviceToHost, e->stream));
   if (e->G && delta_out) CK(e, cudaMemcpyAsync(delta_out, e->delta_slot[slot], e->G, cudaMemcpyDeviceToHost, e->stream));
   CK(e, cudaStreamSynchronize(e->stream));
+  return MRQ_OK;
+}
+
+int mrq_set_change_capacity(mrq_engine *e, uint64_t max_records) {
+  if (!e) return MRQ_E_INVAL;
+  if (max_records > (UINT64_MAX >> 6)) return fail(e, MRQ_E_INVAL, "change capacity %llu is too large", (unsigned long long)max_records);
+  CK(e, cudaSetDevice(e->device));
+  CK(e, cudaStreamSynchronize(e->stream));  // launches in flight may still append to the old buffer
+  // Captured graphs (modes 0-3) hold the old feed arguments: a replay must not run with them, so they start over.  (The
+  // mode-4 descriptor tables hold only frame and output pointers; the feed rides in the kernel arguments of every launch.)
+  for (auto &kv : e->graphs) cudaGraphExecDestroy(kv.second);
+  e->graphs.clear();
+  if (max_records != 0 && max_records == e->change_cap) {  // same size: keep the buffer, discard what is pending
+    CK(e, cudaMemsetAsync(e->change_count, 0, sizeof(unsigned long long), e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    return MRQ_OK;
+  }
+  if (e->changes) CK(e, cudaFree(e->changes));
+  e->changes = nullptr;
+  e->change_cap = 0;
+  if (max_records == 0) return MRQ_OK;
+  if (!e->change_count) {
+    int r = dalloc(e, &e->change_count, 1);
+    if (r) return r;
+  }
+  CK(e, cudaMalloc((void **)&e->changes, max_records * sizeof(mrq_change)));
+  CK(e, cudaMemsetAsync(e->change_count, 0, sizeof(unsigned long long), e->stream));
+  CK(e, cudaStreamSynchronize(e->stream));
+  e->change_cap = max_records;
+  return MRQ_OK;
+}
+
+int mrq_sync_changes(mrq_engine *e, mrq_change *out, uint64_t cap, uint64_t *n_out, uint64_t *lost) {
+  if (!e || !n_out || !lost || (cap && !out)) return MRQ_E_INVAL;
+  if (!e->changes) return fail(e, MRQ_E_STATE, "mrq_sync_changes: the change feed is off (mrq_set_change_capacity)");
+  CK(e, cudaSetDevice(e->device));
+  unsigned long long count = 0;
+  CK(e, cudaMemcpyAsync(&count, e->change_count, sizeof count, cudaMemcpyDeviceToHost, e->stream));
+  CK(e, cudaStreamSynchronize(e->stream));
+  const uint64_t n = count < e->change_cap ? count : e->change_cap;
+  *n_out = n;
+  if (cap < n) {
+    *lost = 0;
+    return fail(e, MRQ_E_INVAL, "mrq_sync_changes: %llu records pending, room for %llu", (unsigned long long)n, (unsigned long long)cap);
+  }
+  if (n) CK(e, cudaMemcpyAsync(out, e->changes, n * sizeof(mrq_change), cudaMemcpyDeviceToHost, e->stream));
+  CK(e, cudaMemsetAsync(e->change_count, 0, sizeof(unsigned long long), e->stream));
+  CK(e, cudaStreamSynchronize(e->stream));
+  // warps append in whatever order they run: the host sorts the (sparse) list
+  std::sort(out, out + n, [](const mrq_change &x, const mrq_change &y) { return x.tick != y.tick ? x.tick < y.tick : x.group < y.group; });
+  *lost = count - n;
   return MRQ_OK;
 }
 

@@ -90,6 +90,11 @@ struct TickArgs {
   // fast/slow split: groups the fast kernel leaves untouched are listed here for the slow kernel
   uint32_t *slow_list;
   unsigned *slow_count, *slow_count_next;
+  // Change feed (mrq_set_change_capacity): the general tick appends one record per group whose term, vote, role or
+  // lead it moved.  change_count counts every record; only the first change_cap are written.  nullptr: feed off.
+  mrq_change *changes;
+  unsigned long long *change_count;
+  uint64_t change_cap;
 };
 
 // ---- programmatic dependent launch (PDL) ---------------------------------------------------------
@@ -623,6 +628,35 @@ __device__ __forceinline__ void count_events(Counters *c, uint32_t ev) {
   }
 }
 
+// Append one change-feed record per lane with what != 0.  Warp-aggregated over the lanes that reach this call (callers
+// run the general tick under divergent guards): one atomic per warp with any change, so a mass election does not
+// serialise one atomic per group on the counter.  Records at or past the capacity are counted, not written.
+__device__ __forceinline__ void append_change(const TickArgs &a, const uint32_t what, const uint64_t tick_no, const uint64_t i,
+                                              const uint64_t term, const uint64_t term_start, const uint32_t vote, const uint32_t role,
+                                              const uint32_t lead) {
+  const unsigned act = __activemask();
+  const unsigned want = __ballot_sync(act, what != 0u);
+  if (what == 0u) return;
+  const unsigned lane = threadIdx.x & 31u;
+  const int leader = __ffs((int)want) - 1;
+  unsigned long long base = 0;
+  if ((int)lane == leader) base = atomicAdd(a.change_count, (unsigned long long)__popc(want));
+  base = __shfl_sync(want, base, leader);
+  const unsigned long long at = base + (unsigned long long)__popc(want & ((1u << lane) - 1u));
+  if (at < a.change_cap) {
+    mrq_change c;
+    c.tick = tick_no;
+    c.term = term;
+    c.term_start = term_start;
+    c.group = (uint32_t)i;
+    c.vote = (uint8_t)vote;
+    c.role = (uint8_t)role;
+    c.lead = (uint8_t)lead;
+    c.what = (uint8_t)what;
+    a.changes[at] = c;
+  }
+}
+
 // ---- the general per-group tick: every message through the full state machine (a3–a16) ------------------
 static constexpr int kTickThreads = 128;
 template <int R>
@@ -689,6 +723,13 @@ __device__ __forceinline__ uint32_t general_group_tick(const TickArgs &a, const 
     }
     st_state_u32(a.s.out + i, g.out);
     if (a.world > 1) gather_store(a, i, g.committed, committed0);  // fused all-gather
+    if (a.changes) {  // HardState {term, vote} / SoftState {lead, role} moved: the change feed
+      // (D_TERM is set exactly when reset() moved the term; role, lead and vote are meta bits [0,2), [2,6), [6,10))
+      const uint32_t d = (uint32_t)(w_new ^ w_meta);
+      const uint32_t what = ((g.dirty & D_TERM) ? MRQ_CHANGE_TERM : 0u) | ((d & 0x3C0u) ? MRQ_CHANGE_VOTE : 0u) |
+                            ((d & 0x3u) ? MRQ_CHANGE_ROLE : 0u) | ((d & 0x3Cu) ? MRQ_CHANGE_LEAD : 0u);
+      append_change(a, what, tick_no, i, g.term, g.role == MRQ_ROLE_LEADER ? g.gate : kNoGate, g.vote, g.role, g.lead);
+    }
     ev = g.ev;
   }
   return ev;

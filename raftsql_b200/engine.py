@@ -55,6 +55,10 @@ def empty_state(G: int, R: int) -> dict:
                 randomized_timeout=np.zeros(G, np.uint16))
 
 
+CHANGE_DTYPE = np.dtype([("tick", np.uint64), ("term", np.uint64), ("term_start", np.uint64), ("group", np.uint32),
+                         ("vote", np.uint8), ("role", np.uint8), ("lead", np.uint8), ("what", np.uint8)])  # mrq_change
+
+
 def empty_inbox(G: int, R: int) -> dict:
     return dict(type=np.zeros((R, G), np.uint8), term=np.zeros((R, G), np.uint64), index=np.zeros((R, G), np.uint64),
                 logterm=np.zeros((R, G), np.uint64), commit=np.zeros((R, G), np.uint64),
@@ -269,6 +273,27 @@ class Engine:
         o, d = np.zeros(self.G, np.uint32), np.zeros(self.G, np.uint8)
         self._ck(self.L.mrq_sync_slot_outputs(self.h, slot, _p(o, F.u32p), _p(d, F.u8p)))
         return o, d
+
+    def set_change_capacity(self, n: int):
+        """Change feed: record up to n changes of term / vote / role / lead between drains (0 = off).  Discards
+        pending records."""
+        self._ck(self.L.mrq_set_change_capacity(self.h, n))
+        self._change_room = min(int(n), 1 << 16)
+
+    def sync_changes(self):
+        """Drain the change feed: (records sorted by (tick, group) as a CHANGE_DTYPE array, lost).  lost > 0 means
+        the list is incomplete and the host must read state in full."""
+        room = max(1, getattr(self, "_change_room", 1))
+        n, lost = C.c_uint64(), C.c_uint64()
+        while True:
+            buf = np.zeros(room, CHANGE_DTYPE)
+            rc = self.L.mrq_sync_changes(self.h, buf.ctypes.data_as(C.POINTER(F.Change)), room, C.byref(n), C.byref(lost))
+            if rc == F.MRQ_E_INVAL and n.value > room:  # more records than room: nothing was consumed, retry with enough
+                room = int(n.value)
+                continue
+            self._ck(rc)
+            self._change_room = room
+            return buf[: n.value], int(lost.value)
 
     def counters(self) -> dict:
         c = F.Counters()
