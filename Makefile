@@ -89,11 +89,20 @@ tests/cpp/change_feed_host_test: $(FEEDHOST_DEP)
 tests/cpp/change_feed_host_test_san: $(FEEDHOST_DEP)
 	$(SAN_CXX) -std=c++17 -O0 -fsanitize=address,undefined -fno-sanitize-recover=undefined -I$(CUDA_INC) -pthread -o $@ $(FEEDHOST_SRC)
 
+# The state of a list of groups: export_group_row / import_group_row over mode-4 states reached by traces and soups,
+# against materialise_group and the oracle (it includes tick_host_test.cpp for the harness).
+GROUPHOST_SRC := tests/cpp/group_state_host_test.cpp oracle/raft_oracle.c
+GROUPHOST_DEP := $(GROUPHOST_SRC) $(TICKHOST_DEP)
+tests/cpp/group_state_host_test: $(GROUPHOST_DEP)
+	$(CXX) -std=c++17 -O1 -I$(CUDA_INC) -pthread -o $@ $(GROUPHOST_SRC)
+tests/cpp/group_state_host_test_san: $(GROUPHOST_DEP)
+	$(SAN_CXX) -std=c++17 -O0 -fsanitize=address,undefined -fno-sanitize-recover=undefined -I$(CUDA_INC) -pthread -o $@ $(GROUPHOST_SRC)
+
 clean:
 	rm -f $(LIB) $(HOSTLIB) $(CPPTEST) tests/cpp/raftpipe_test_asan tests/cpp/raftpipe_test_tsan build_ptxas.log \
 	  tests/cpp/tick_host_test tests/cpp/tick_host_test_san tests/cpp/tick_host16_test tests/cpp/tick_host16_test_san \
 	  tests/cpp/tick_clock_host_test tests/cpp/tick_clock_host_test_san tests/cpp/tick_pair_host_test tests/cpp/tick_pair_host_test_san \
 	  tests/cpp/tick_pair_clock_host_test tests/cpp/tick_pair_clock_host_test_san \
-	  tests/cpp/change_feed_host_test tests/cpp/change_feed_host_test_san
+	  tests/cpp/change_feed_host_test tests/cpp/change_feed_host_test_san tests/cpp/group_state_host_test tests/cpp/group_state_host_test_san
 	$(MAKE) -C oracle clean
 .PHONY: all oracle clean san_cxx

@@ -345,3 +345,95 @@ func (e *Engine) SyncChanges() (changes []Change, lost uint64, err error) {
 	}
 	return changes, uint64(l), nil
 }
+
+// GroupState holds rows of listed groups: [n] per column, [R*n] replica-major for Match and Votes (element r*n+k
+// belongs to groups[k]).  A nil column is skipped.
+type GroupState struct {
+	Term, Vote, Committed, LastIndex, LastTerm, TermStart, Match []uint64
+	Role, Lead, SelfID, Votes                                    []uint8
+	ElectionElapsed, HeartbeatElapsed, RandomizedTimeout         []uint16
+}
+
+// cState lays the non-nil columns of s out in C memory (cgo: a struct handed to C must not hold Go pointers) and
+// returns the mrq_state over them, a copy-back for exports, and the free.
+func (s *GroupState) cState(copyIn bool) (st C.mrq_state, copyBack func(), free func()) {
+	var bufs []unsafe.Pointer
+	var backs []func()
+	col := func(p unsafe.Pointer, n int, size uintptr) unsafe.Pointer {
+		if n == 0 {
+			return nil
+		}
+		c := C.malloc(C.size_t(uintptr(n) * size))
+		bufs = append(bufs, c)
+		dst, src := unsafe.Slice((*byte)(c), uintptr(n)*size), unsafe.Slice((*byte)(p), uintptr(n)*size)
+		if copyIn {
+			copy(dst, src)
+		}
+		backs = append(backs, func() { copy(src, dst) })
+		return c
+	}
+	u64 := func(v []uint64) *C.uint64_t {
+		if len(v) == 0 {
+			return nil
+		}
+		return (*C.uint64_t)(col(unsafe.Pointer(&v[0]), len(v), 8))
+	}
+	u8 := func(v []uint8) *C.uint8_t {
+		if len(v) == 0 {
+			return nil
+		}
+		return (*C.uint8_t)(col(unsafe.Pointer(&v[0]), len(v), 1))
+	}
+	u16 := func(v []uint16) *C.uint16_t {
+		if len(v) == 0 {
+			return nil
+		}
+		return (*C.uint16_t)(col(unsafe.Pointer(&v[0]), len(v), 2))
+	}
+	st.term, st.vote, st.committed, st.last_index = u64(s.Term), u64(s.Vote), u64(s.Committed), u64(s.LastIndex)
+	st.last_term, st.term_start, st.match = u64(s.LastTerm), u64(s.TermStart), u64(s.Match)
+	st.role, st.lead, st.self_id, st.votes = u8(s.Role), u8(s.Lead), u8(s.SelfID), u8(s.Votes)
+	st.election_elapsed, st.heartbeat_elapsed, st.randomized_timeout = u16(s.ElectionElapsed), u16(s.HeartbeatElapsed), u16(s.RandomizedTimeout)
+	copyBack = func() {
+		for _, b := range backs {
+			b()
+		}
+	}
+	free = func() {
+		for _, b := range bufs {
+			C.free(b)
+		}
+	}
+	return
+}
+
+// ExportGroups reads the rows of the listed local groups (duplicates allowed) into the non-nil columns of out, each
+// sized for len(groups) rows: row k is exactly column groups[k] of a whole-engine export.  It writes no engine state
+// and converts no representation, so it costs what n groups cost — e.g. the groups whose commit advance saturated at
+// 255, or a status lookup.
+func (e *Engine) ExportGroups(groups []uint64, out *GroupState) error {
+	if len(groups) == 0 {
+		return nil
+	}
+	st, copyBack, free := out.cState(false)
+	defer free()
+	if rc := C.mrq_export_groups(e.h, (*C.uint64_t)(unsafe.Pointer(&groups[0])), C.uint64_t(len(groups)), &st); rc != 0 {
+		return lastErr(e.h)
+	}
+	copyBack()
+	return nil
+}
+
+// ImportGroups overwrites the non-nil columns of the listed local groups (no duplicates) — e.g. one group replayed
+// from its WAL — leaving every other group, and its compact state in tick mode 4, untouched.
+func (e *Engine) ImportGroups(groups []uint64, in *GroupState) error {
+	if len(groups) == 0 {
+		return nil
+	}
+	st, _, free := in.cState(true)
+	defer free()
+	if rc := C.mrq_import_groups(e.h, (*C.uint64_t)(unsafe.Pointer(&groups[0])), C.uint64_t(len(groups)), &st); rc != 0 {
+		return lastErr(e.h)
+	}
+	return nil
+}

@@ -125,6 +125,24 @@ typedef struct mrq_state {
 
 int mrq_export_state(mrq_engine *e, mrq_state *out); /* blocking: device -> caller arrays      */
 int mrq_import_state(mrq_engine *e, const mrq_state *in); /* blocking: caller arrays -> device */
+/* The same for a list of local groups, at a cost that follows n, not G (one kernel launch plus the copies).
+ * `out` / `in` are mrq_state with n-row arrays: [n], and [R][n] for match / votes (element [r * n + k] belongs to
+ * groups[k]); a NULL pointer skips that column.  n == 0: no-op.  groups == NULL with n > 0: MRQ_E_INVAL.  G == 0: OK.
+ * Neither call records change-feed entries (as mrq_import_state: the feed does not record the host's own changes),
+ * moves the mrq_sync_commit_deltas drain base (only mrq_sync_commits rebases it), or invalidates captured CUDA graphs
+ * or mode-4 descriptor tables (only device memory contents change).
+ *
+ * mrq_export_groups: blocking.  Row k is exactly row groups[k] of what mrq_export_state would return at that point.
+ * Duplicates are allowed.  Writes no engine state and converts no representation (tick mode 4's compact groups are
+ * decoded in the kernel); a group >= G: MRQ_E_INVAL.
+ * mrq_import_groups: blocking.  Overwrites the given columns of the listed groups, with the same effect on them as
+ * "export everything, overwrite those rows, import everything" — on every later export, out word, commit advance,
+ * change-feed record and counter except kernel_launches.  The other groups' state, including their compact
+ * representation in tick mode 4, is untouched (unlike mrq_import_state, whose whole-engine conversion makes the next
+ * mode-4 tick re-compact every group).  A duplicate or a group >= G: MRQ_E_INVAL, nothing changed.  With the fused
+ * gather on (mrq_comm_set_mode(1)) an import of `committed` makes the next tick republish every full index.  */
+int mrq_export_groups(mrq_engine *e, const uint64_t *groups, uint64_t n, mrq_state *out);
+int mrq_import_groups(mrq_engine *e, const uint64_t *groups, uint64_t n, const mrq_state *in);
 /* Progress.Next is message-construction state; without rejections it is exactly
  * max(term_start, match+1) (reset() sets Next = lastIndex+1 == term_start; maybeUpdate raises it
  * to n+1).  Exported as a convenience for the host's sendAppend.  out is [R][G].              */

@@ -114,6 +114,8 @@ SIGNATURES = {
     "mrq_last_error": (C.c_char_p, [_EP]),
     "mrq_export_state": (C.c_int, [_EP, C.POINTER(State)]),
     "mrq_import_state": (C.c_int, [_EP, C.POINTER(State)]),
+    "mrq_export_groups": (C.c_int, [_EP, u64p, C.c_uint64, C.POINTER(State)]),
+    "mrq_import_groups": (C.c_int, [_EP, u64p, C.c_uint64, C.POINTER(State)]),
     "mrq_export_next": (C.c_int, [_EP, u64p]),
     "mrq_tick_count": (C.c_uint64, [_EP]),
     "mrq_set_tick_count": (C.c_int, [_EP, C.c_uint64]),

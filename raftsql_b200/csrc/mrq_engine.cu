@@ -852,6 +852,132 @@ int mrq_import_state(mrq_engine *e, const mrq_state *in) {
   return MRQ_OK;
 }
 
+// ---- state of a list of groups ------------------------------------------------------------------------------
+namespace {
+
+int ensure_pinned(mrq_engine *e, size_t bytes) {
+  if (bytes <= e->pinned_bytes) return MRQ_OK;
+  if (e->pinned) {
+    CK(e, cudaStreamSynchronize(e->stream));
+    CK(e, cudaFreeHost(e->pinned));
+    e->pinned = nullptr;
+    e->pinned_bytes = 0;
+  }
+  const size_t want = bytes < (1u << 20) ? (1u << 20) : bytes;
+  if (cudaHostAlloc(&e->pinned, want, cudaHostAllocDefault) != cudaSuccess) {
+    cudaGetLastError();
+    e->pinned = nullptr;
+    return fail(e, MRQ_E_NOMEM, "cannot allocate %zu bytes of page-locked staging", want);
+  }
+  e->pinned_bytes = want;
+  return MRQ_OK;
+}
+
+// The columns of an n-row mrq_state, in GroupRows order, laid out in one staging block behind the n group ids: the
+// block goes to / comes from the device in one copy, and the device pointers of the columns that are not NULL make
+// the kernel's GroupRows (NULL columns get no room and stay NULL there).
+struct RowsLayout {
+  static constexpr int kCols = 14;
+  void *host[kCols];
+  size_t off[kCols], bytes[kCols];
+  size_t cols_begin, total;
+  RowsLayout(const mrq_state *st, uint64_t n, uint32_t R) {
+    void *const h[kCols] = {st->term,  st->vote,    st->committed, st->last_index, st->last_term,        st->term_start,        st->match,
+                            st->role,  st->lead,    st->self_id,   st->votes,      st->election_elapsed, st->heartbeat_elapsed, st->randomized_timeout};
+    static const size_t elem[kCols] = {8, 8, 8, 8, 8, 8, 8, 1, 1, 1, 1, 2, 2, 2};
+    static const bool per_replica[kCols] = {false, false, false, false, false, false, true, false, false, false, true, false, false, false};
+    size_t at = ((n * 8 + 15) / 16) * 16;
+    cols_begin = at;
+    for (int k = 0; k < kCols; ++k) {
+      host[k] = h[k];
+      bytes[k] = h[k] ? elem[k] * n * (per_replica[k] ? R : 1u) : 0;
+      off[k] = at;
+      at += ((bytes[k] + 15) / 16) * 16;
+    }
+    total = at;
+  }
+  GroupRows rows(uint8_t *dev) const {
+    auto p = [&](int k) -> void * { return host[k] ? dev + off[k] : nullptr; };
+    return GroupRows{(uint64_t *)p(0), (uint64_t *)p(1), (uint64_t *)p(2), (uint64_t *)p(3), (uint64_t *)p(4),
+                     (uint64_t *)p(5), (uint64_t *)p(6), (uint8_t *)p(7),  (uint8_t *)p(8),  (uint8_t *)p(9),
+                     (uint8_t *)p(10), (uint16_t *)p(11), (uint16_t *)p(12), (uint16_t *)p(13)};
+  }
+};
+
+// Shared argument checks of the group-list calls.  MRQ_OK with *skip set: nothing to do (n == 0, or G == 0).
+int check_group_list(mrq_engine *e, const uint64_t *groups, uint64_t n, bool unique, bool *skip) {
+  *skip = true;
+  if (n == 0) return MRQ_OK;
+  if (!groups) return fail(e, MRQ_E_INVAL, "null group list with n = %llu", (unsigned long long)n);
+  if (e->G == 0) return MRQ_OK;
+  for (uint64_t k = 0; k < n; ++k)
+    if (groups[k] >= e->G)
+      return fail(e, MRQ_E_INVAL, "group %llu (list entry %llu) out of range: G = %llu", (unsigned long long)groups[k], (unsigned long long)k,
+                  (unsigned long long)e->G);
+  if (unique) {  // one thread per listed group writes that group: a duplicate would race with itself
+    std::vector<uint64_t> sorted(groups, groups + n);
+    std::sort(sorted.begin(), sorted.end());
+    const auto d = std::adjacent_find(sorted.begin(), sorted.end());
+    if (d != sorted.end()) return fail(e, MRQ_E_INVAL, "group %llu is listed twice", (unsigned long long)*d);
+  }
+  *skip = false;
+  return MRQ_OK;
+}
+
+}  // namespace
+
+int mrq_export_groups(mrq_engine *e, const uint64_t *groups, uint64_t n, mrq_state *out) {
+  if (!e || !out) return MRQ_E_INVAL;
+  bool skip;
+  int r = check_group_list(e, groups, n, false, &skip);
+  if (r || skip) return r;
+  CK(e, cudaSetDevice(e->device));
+  const RowsLayout L(out, n, e->R);
+  if ((r = ensure_scratch(e, L.total)) || (r = ensure_pinned(e, L.total))) return r;
+  uint8_t *dev = (uint8_t *)e->scratch, *pin = (uint8_t *)e->pinned;
+  memcpy(pin, groups, n * 8);
+  CK(e, cudaMemcpyAsync(dev, pin, n * 8, cudaMemcpyHostToDevice, e->stream));
+  const bool compact = e->compact_live;
+  export_groups_kernel<<<nblocks(n), 256, 0, e->stream>>>(e->s, e->c, compact ? 1 : 0, e->gs, e->R, (const uint64_t *)dev, n, e->tick_no,
+                                                          e->cfg.election_tick, e->cfg.heartbeat_tick, L.rows(dev));
+  CK(e, cudaGetLastError());
+  e->launches++;
+  if (L.total > L.cols_begin)
+    CK(e, cudaMemcpyAsync(pin + L.cols_begin, dev + L.cols_begin, L.total - L.cols_begin, cudaMemcpyDeviceToHost, e->stream));
+  CK(e, cudaStreamSynchronize(e->stream));
+  for (int k = 0; k < RowsLayout::kCols; ++k)
+    if (L.host[k]) memcpy(L.host[k], pin + L.off[k], L.bytes[k]);
+  return MRQ_OK;
+}
+
+int mrq_import_groups(mrq_engine *e, const uint64_t *groups, uint64_t n, const mrq_state *in) {
+  if (!e || !in) return MRQ_E_INVAL;
+  bool skip;
+  int r = check_group_list(e, groups, n, true, &skip);
+  if (r || skip) return r;
+  CK(e, cudaSetDevice(e->device));
+  const RowsLayout L(in, n, e->R);
+  if ((r = ensure_scratch(e, L.total)) || (r = ensure_pinned(e, L.total))) return r;
+  uint8_t *dev = (uint8_t *)e->scratch, *pin = (uint8_t *)e->pinned;
+  memcpy(pin, groups, n * 8);
+  for (int k = 0; k < RowsLayout::kCols; ++k)
+    if (L.host[k]) memcpy(pin + L.off[k], L.host[k], L.bytes[k]);
+  CK(e, cudaMemcpyAsync(dev, pin, L.total, cudaMemcpyHostToDevice, e->stream));
+  // With the compact state live the kernel materialises and re-compacts exactly the listed groups; every other group
+  // keeps its compact copy, so the next mode-4 launch needs no compact_all_kernel.
+  const bool compact = e->compact_live;
+  import_groups_kernel<<<nblocks(n), 256, 0, e->stream>>>(e->s, e->c, compact ? 1 : 0, e->pk_base_index, e->pk_base_term, e->gs, e->R,
+                                                          (const uint64_t *)dev, n, e->tick_no, e->cfg.election_tick,
+                                                          e->cfg.heartbeat_tick, L.rows(dev));
+  CK(e, cudaGetLastError());
+  e->launches++;
+  // The fused gather stores a group's full index only when its high bits move during a tick: an imported index has to
+  // be republished in full, or the peers would stitch the old high bits onto its new low byte.
+  if (in->committed && e->comm_mode == 1) e->gather_prime = true;
+  CK(e, cudaStreamSynchronize(e->stream));
+  return MRQ_OK;
+}
+
 int mrq_export_next(mrq_engine *e, uint64_t *next_out) {
   if (!e || !next_out) return MRQ_E_INVAL;
   CK(e, cudaSetDevice(e->device));

@@ -1648,30 +1648,52 @@ __device__ __forceinline__ bool compact_step(CGroup<R> &g, const uint32_t flag, 
   return false;
 }
 
+// The wide values of a COMPACT group i, decoded from its compact columns and handed one by one to put(column, replica
+// slot, value) — the columns the compact form holds differently: meta (only a leader's, whose real timers come from
+// c.clk against `T`, the number of the next tick to run), committed, the window base, lastIndex, and the Match entries
+// the compact form knows (a leader's own = lastIndex; a zero offset means the wide value, <= ibase, stands, and is not
+// handed over).  Every other wide column is already exact.  materialise_group stores the values; the group-list export
+// (export_group_row) reads them without writing any engine state.  Reads and stores interleave in the order of the
+// former single function, so materialise_group compiles as it did.
+enum : uint32_t { WV_META, WV_COMMITTED, WV_WINDOW, WV_LAST_INDEX, WV_MATCH };
+template <typename Off, typename Put>
+__device__ __forceinline__ void decode_compact_group(const StateView &s, const CompactViewT<Off> &c, uint64_t gs, uint32_t R, const uint64_t i,
+                                                     const uint64_t T, const uint32_t et, const uint32_t ht, Put &&put) {
+  Meta m = meta_unpack(s.meta[i]);
+  if (c.clk && m.role == MRQ_ROLE_LEADER) {
+    const uint32_t p = c.clk[i];
+    m.elapsed = clk_value(p & 0xFFFFu, T, et);
+    m.hb = clk_value((p >> 16) & 0xFFu, T, ht);
+    put(WV_META, 0u, meta_pack(m));
+  }
+  const uint64_t ib = c.ibase[i];
+  put(WV_COMMITTED, 0u, ib + c.commit[i]);
+  put(WV_WINDOW, 0u, ib + c.win[i]);
+  put(WV_LAST_INDEX, 0u, ib + c.match[(uint64_t)(R - 1u) * gs + i]);
+  if (m.role == MRQ_ROLE_LEADER) {
+    put(WV_MATCH, m.self - 1u, ib + c.match[(uint64_t)(R - 1u) * gs + i]);  // a leader's own Match is lastIndex
+    for (uint32_t j = 0; j + 1u < R; ++j) {
+      const uint32_t v = c.match[(uint64_t)j * gs + i];
+      if (v != 0u) put(WV_MATCH, crow_sender(j, m.self), ib + v);  // 0: the wide value (<= ibase) stands
+    }
+  }
+}
+
 // compact -> wide for one group: the wide columns become exact copies (flag and c.clk untouched).  With c.clk, `T` is
 // the number of the next tick to run and a leader's real timers are written into meta.
 template <typename Off>
 __device__ __forceinline__ void materialise_group(const StateView &s, const CompactViewT<Off> &c, uint64_t *base_index, uint64_t gs, uint32_t R,
                                                   const uint64_t i, const uint64_t T = 0, const uint32_t et = 1, const uint32_t ht = 1) {
   if (!(c.flag[i] & CF_COMPACT)) return;
-  Meta m = meta_unpack(s.meta[i]);
-  if (c.clk && m.role == MRQ_ROLE_LEADER) {
-    const uint32_t p = c.clk[i];
-    m.elapsed = clk_value(p & 0xFFFFu, T, et);
-    m.hb = clk_value((p >> 16) & 0xFFu, T, ht);
-    s.meta[i] = meta_pack(m);
-  }
-  const uint64_t ib = c.ibase[i];
-  s.committed[i] = ib + c.commit[i];
-  base_index[i] = ib + c.win[i];
-  s.last_index[i] = ib + c.match[(uint64_t)(R - 1u) * gs + i];
-  if (m.role == MRQ_ROLE_LEADER) {
-    s.match[(uint64_t)(m.self - 1u) * gs + i] = ib + c.match[(uint64_t)(R - 1u) * gs + i];  // a leader's own Match is lastIndex
-    for (uint32_t j = 0; j + 1u < R; ++j) {
-      const uint32_t v = c.match[(uint64_t)j * gs + i];
-      if (v != 0u) s.match[(uint64_t)crow_sender(j, m.self) * gs + i] = ib + v;  // 0: the wide value (<= ibase) stands
+  decode_compact_group(s, c, gs, R, i, T, et, ht, [&](const uint32_t col, const uint32_t r, const uint64_t v) {
+    switch (col) {
+      case WV_META: s.meta[i] = v; break;
+      case WV_COMMITTED: s.committed[i] = v; break;
+      case WV_WINDOW: base_index[i] = v; break;
+      case WV_LAST_INDEX: s.last_index[i] = v; break;
+      default: s.match[(uint64_t)r * gs + i] = v; break;
     }
-  }
+  });
 }
 
 // wide -> compact for one group (after the general path, an import, or a new window base): picks a fresh ibase just
@@ -1715,6 +1737,96 @@ __device__ __forceinline__ void compact_group(const StateView &s, const CompactV
   if (leader) go = gate > ib ? (gate - ib >= (uint64_t)kClosed ? kClosed : (Off)(gate - ib)) : (Off)0;
   c.gate[i] = go;
   c.flag[i] = (uint8_t)(CF_COMPACT | (base_term[i] == s.term[i] ? CF_TERM_OK : 0u) | ((leader && gate <= cm) ? CF_GATE_OPEN : 0u));
+}
+
+// ---- rows of a list of groups (mrq_export_groups / mrq_import_groups) --------------------------------------------------
+// The columns of mrq_state with n rows instead of G: row k belongs to the k-th listed group; match and votes are
+// [R][n].  A null column is neither written (export) nor read (import).
+struct GroupRows {
+  uint64_t *term, *vote, *committed, *last_index, *last_term, *term_start, *match;
+  uint8_t *role, *lead, *self_id, *votes;
+  uint16_t *el, *hb, *rto;
+};
+
+// Row k of an export: group i exactly as mrq_export_state returns it (the wide columns, the compact ones decoded where
+// the group is compact, meta unpacked as unpack_meta_kernel does).  `compact`: the engine's compact state is live (c is
+// read only then).  Writes nothing but the row: no engine state, no representation change.
+template <typename Off>
+__device__ __forceinline__ void export_group_row(const StateView &s, const CompactViewT<Off> &c, const bool compact, uint64_t gs, uint32_t R,
+                                                 const uint64_t i, const uint64_t T, const uint32_t et, const uint32_t ht, const GroupRows &o,
+                                                 const uint64_t n, const uint64_t k) {
+  uint64_t meta = s.meta[i], committed = s.committed[i], li = s.last_index[i];
+  if (o.match)
+    for (uint32_t r = 0; r < R; ++r) o.match[(uint64_t)r * n + k] = s.match[(uint64_t)r * gs + i];
+  if (compact && (c.flag[i] & CF_COMPACT))
+    decode_compact_group(s, c, gs, R, i, T, et, ht, [&](const uint32_t col, const uint32_t r, const uint64_t v) {
+      switch (col) {
+        case WV_META: meta = v; break;
+        case WV_COMMITTED: committed = v; break;
+        case WV_WINDOW: break;  // (the packed-inbox window base is not part of mrq_state)
+        case WV_LAST_INDEX: li = v; break;
+        default:
+          if (o.match) o.match[(uint64_t)r * n + k] = v;
+          break;
+      }
+    });
+  const Meta m = meta_unpack(meta);
+  if (o.term) o.term[k] = s.term[i];
+  if (o.vote) o.vote[k] = m.vote;
+  if (o.committed) o.committed[k] = committed;
+  if (o.last_index) o.last_index[k] = li;
+  if (o.last_term) o.last_term[k] = s.last_term[i];
+  if (o.term_start) o.term_start[k] = s.term_start[i];
+  if (o.role) o.role[k] = (uint8_t)m.role;
+  if (o.lead) o.lead[k] = (uint8_t)m.lead;
+  if (o.self_id) o.self_id[k] = (uint8_t)m.self;
+  if (o.el) o.el[k] = (uint16_t)m.elapsed;
+  if (o.hb) o.hb[k] = (uint16_t)m.hb;
+  if (o.rto) o.rto[k] = (uint16_t)m.rto;
+  if (o.votes)
+    for (uint32_t r = 0; r < R; ++r) o.votes[(uint64_t)r * n + k] = (uint8_t)((m.votes >> (2 * r)) & 3u);
+}
+
+// Row k of an import into group i: what mrq_import_state does to that group, and nothing to any other.  A compact group
+// is materialised first (`T`: the number of the next tick to run); then the given wide columns are overwritten and the
+// given meta fields packed (pack_meta_kernel's rules), strict and ltok recomputed (fix_strict_kernel's rule), and, with
+// the compact state live, the group re-compacted at T — a group that does not fit gets flag 0 and takes the general path
+// on its next mode-4 tick, as after a whole-engine import.
+template <typename Off>
+__device__ __forceinline__ void import_group_row(const StateView &s, const CompactViewT<Off> &c, const bool compact, uint64_t *base_index,
+                                                 const uint64_t *base_term, uint64_t gs, uint32_t R, const uint64_t i, const uint64_t T,
+                                                 const uint32_t et, const uint32_t ht, const GroupRows &in, const uint64_t n, const uint64_t k) {
+  if (compact) materialise_group(s, c, base_index, gs, R, i, T, et, ht);
+  if (in.term) s.term[i] = in.term[k];
+  if (in.committed) s.committed[i] = in.committed[k];
+  if (in.last_index) s.last_index[i] = in.last_index[k];
+  if (in.last_term) s.last_term[i] = in.last_term[k];
+  if (in.term_start) s.term_start[i] = in.term_start[k];
+  if (in.match)
+    for (uint32_t r = 0; r < R; ++r) s.match[(uint64_t)r * gs + i] = in.match[(uint64_t)r * n + k];
+  Meta m = meta_unpack(s.meta[i]);
+  if (in.role) m.role = in.role[k];
+  if (in.lead) m.lead = in.lead[k];
+  if (in.self_id) m.self = in.self_id[k];
+  if (in.vote) m.vote = (uint32_t)in.vote[k];
+  if (in.el) m.elapsed = in.el[k];
+  if (in.hb) m.hb = in.hb[k];
+  if (in.rto) m.rto = in.rto[k];
+  if (in.votes) {
+    uint32_t w = 0;
+    for (uint32_t r = 0; r < R; ++r) w |= (uint32_t)(in.votes[(uint64_t)r * n + k] & 3u) << (2 * r);
+    m.votes = w;
+  }
+  m = meta_unpack(meta_pack(m));  // the fields as stored (an out-of-range role is masked before the strict rule reads it)
+  uint32_t strict = 0;
+  if (m.role == MRQ_ROLE_LEADER) {
+    const uint64_t li = s.last_index[i];
+    for (uint32_t r = 0; r < R; ++r) strict |= s.match[(uint64_t)r * gs + i] > li;
+  }
+  m.strict = strict;
+  m.ltok = s.last_term[i] == s.term[i];
+  s.meta[i] = meta_pack(m);
+  if (compact) compact_group(s, c, base_index, base_term, gs, R, i, T, et, ht);
 }
 
 // One tick of a mode-4 launch: where its frame is, and where its per-tick outputs go.
@@ -2261,6 +2373,23 @@ __global__ void __launch_bounds__(256) compact_all_kernel(StateView s, CompactVi
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= G) return;
   compact_group(s, c, base_index, base_term, gs, R, i, T, et, ht);
+}
+
+// mrq_export_groups / mrq_import_groups: one thread per listed group (the host has checked the list: every group < G,
+// and no duplicate in an import, so no two threads of an import touch one group).  `compact`: the compact state is live.
+__global__ void __launch_bounds__(256) export_groups_kernel(StateView s, CompactViewT<CompactOff> c, int compact, uint64_t gs, uint32_t R,
+                                                             const uint64_t *groups, uint64_t n, uint64_t T, uint32_t et, uint32_t ht,
+                                                             GroupRows o) {
+  const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  export_group_row(s, c, compact != 0, gs, R, groups[k], T, et, ht, o, n, k);
+}
+__global__ void __launch_bounds__(256) import_groups_kernel(StateView s, CompactViewT<CompactOff> c, int compact, uint64_t *base_index,
+                                                             const uint64_t *base_term, uint64_t gs, uint32_t R, const uint64_t *groups,
+                                                             uint64_t n, uint64_t T, uint32_t et, uint32_t ht, GroupRows in) {
+  const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  import_group_row(s, c, compact != 0, base_index, base_term, gs, R, groups[k], T, et, ht, in, n, k);
 }
 #endif  // !MRQ_HOST_EMULATION
 

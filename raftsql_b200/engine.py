@@ -126,6 +126,37 @@ class Engine:
                 setattr(st, k, _p(a, ty))
         self._ck(self.L.mrq_import_state(self.h, C.byref(st)))
 
+    def export_groups(self, groups, columns=STATE_COLUMNS) -> dict:
+        """Rows of the listed local groups (duplicates allowed): arrays of shape [n], and [R, n] for match / votes.
+        Row k equals column groups[k] of export_state(); nothing in the engine changes or converts."""
+        g = np.ascontiguousarray(groups, dtype=np.uint64).reshape(-1)
+        rows = empty_state(len(g), self.R)
+        st = F.State()
+        out = {}
+        for k in columns:
+            setattr(st, k, _p(rows[k], _STATE_TYPES[k]))
+            out[k] = rows[k]
+        self._ck(self.L.mrq_export_groups(self.h, _p(g, F.u64p), len(g), C.byref(st)))
+        return out
+
+    def import_groups(self, groups, s: dict):
+        """Overwrite the given columns of the listed local groups (no duplicates) with rows shaped as export_groups
+        returns them; every other group, including its compact state in tick mode 4, is untouched."""
+        g = np.ascontiguousarray(groups, dtype=np.uint64).reshape(-1)
+        st = F.State()
+        keep = []
+        for k, ty in _STATE_TYPES.items():
+            a = s.get(k)
+            if a is not None:
+                dt = np.dtype(ty._type_)
+                a = np.ascontiguousarray(a, dtype=dt)
+                want = (self.R, len(g)) if k in ("match", "votes") else (len(g),)
+                if a.shape != want:
+                    raise ValueError(f"{k}: shape {a.shape}, want {want}")
+                keep.append(a)
+                setattr(st, k, _p(a, ty))
+        self._ck(self.L.mrq_import_groups(self.h, _p(g, F.u64p), len(g), C.byref(st)))
+
     def export_next(self) -> np.ndarray:
         nx = np.zeros((self.R, self.G), np.uint64)
         self._ck(self.L.mrq_export_next(self.h, _p(nx, F.u64p)))
