@@ -98,11 +98,20 @@ tests/cpp/group_state_host_test: $(GROUPHOST_DEP)
 tests/cpp/group_state_host_test_san: $(GROUPHOST_DEP)
 	$(SAN_CXX) -std=c++17 -O0 -fsanitize=address,undefined -fno-sanitize-recover=undefined -I$(CUDA_INC) -pthread -o $@ $(GROUPHOST_SRC)
 
+# The fresh groups of mrq_resize_groups: init_state_kernel's rows against create's and the oracle's, for R = 1..8.
+RESIZEHOST_SRC := tests/cpp/resize_host_test.cpp oracle/raft_oracle.c
+RESIZEHOST_DEP := $(RESIZEHOST_SRC) tests/cpp/device_on_host.hpp oracle/raft_oracle.h $(HDR)
+tests/cpp/resize_host_test: $(RESIZEHOST_DEP)
+	$(CXX) -std=c++17 -O1 -I$(CUDA_INC) -pthread -o $@ $(RESIZEHOST_SRC)
+tests/cpp/resize_host_test_san: $(RESIZEHOST_DEP)
+	$(SAN_CXX) -std=c++17 -O0 -fsanitize=address,undefined -fno-sanitize-recover=undefined -I$(CUDA_INC) -pthread -o $@ $(RESIZEHOST_SRC)
+
 clean:
 	rm -f $(LIB) $(HOSTLIB) $(CPPTEST) tests/cpp/raftpipe_test_asan tests/cpp/raftpipe_test_tsan build_ptxas.log \
 	  tests/cpp/tick_host_test tests/cpp/tick_host_test_san tests/cpp/tick_host16_test tests/cpp/tick_host16_test_san \
 	  tests/cpp/tick_clock_host_test tests/cpp/tick_clock_host_test_san tests/cpp/tick_pair_host_test tests/cpp/tick_pair_host_test_san \
 	  tests/cpp/tick_pair_clock_host_test tests/cpp/tick_pair_clock_host_test_san \
-	  tests/cpp/change_feed_host_test tests/cpp/change_feed_host_test_san tests/cpp/group_state_host_test tests/cpp/group_state_host_test_san
+	  tests/cpp/change_feed_host_test tests/cpp/change_feed_host_test_san tests/cpp/group_state_host_test tests/cpp/group_state_host_test_san \
+	  tests/cpp/resize_host_test tests/cpp/resize_host_test_san
 	$(MAKE) -C oracle clean
 .PHONY: all oracle clean san_cxx

@@ -437,3 +437,15 @@ func (e *Engine) ImportGroups(groups []uint64, in *GroupState) error {
 	}
 	return nil
 }
+
+// ResizeGroups makes the engine hold n groups — fresh followers added at the tail, or the last groups dropped — as
+// ranges split, merge or move on and off this node.  The other groups keep their state (and their compact form in tick
+// mode 4); every inbox slot is cleared.  Slices sized by the group count take n elements from here on.  An engine with
+// a communicator or CUDA-IPC gather attached refuses it.
+func (e *Engine) ResizeGroups(n uint64) error {
+	if rc := C.mrq_resize_groups(e.h, C.uint64_t(n)); rc != 0 {
+		return lastErr(e.h)
+	}
+	e.g = n
+	return nil
+}

@@ -150,6 +150,28 @@ int mrq_export_next(mrq_engine *e, uint64_t *next_out);
 uint64_t mrq_tick_count(const mrq_engine *e);
 int mrq_set_tick_count(mrq_engine *e, uint64_t t);
 
+/* Blocking.  Make the engine hold n_groups groups: add fresh groups at the tail or drop the last ones, as ranges split,
+ * merge, or move on and off this node, without recreating the engine.
+ * - Groups g < min(old, new) keep every column of mrq_export_state and mrq_export_next, their mrq_sync_commit_deltas
+ *   drain base, their packed decode bases (including a base the device slid), and in tick mode 4 their compact form:
+ *   no whole-engine conversion, and the next tick re-compacts nothing.
+ * - Groups old <= g < new are exactly the rows mrq_create with this config and n_groups = new makes: followers at term
+ *   0 with an empty log, term_start UINT64_MAX, self id by the rotate rule on group_base + g when self_id == 0, the
+ *   randomized timeout drawn as at create (tick key 0), packed bases 0, drain base 0.
+ * - Groups new <= g < old are gone.
+ * - Kept: the tick count, counters, tick / graph mode, L2 policy, quorum variant, write-through, the change-feed
+ *   capacity and its pending records (records naming dropped groups included: they describe ticks that happened).
+ * - Reset as after mrq_create: every inbox slot is cleared (MRQ_PACKED_KEEP frames too; the call waits for the copy
+ *   stream first); mrq_sync_out, mrq_sync_slot_outputs and mrq_drain_tick_deltas behave as right after mrq_create until
+ *   the next tick.  Captured graphs are dropped, and mode-4 descriptor tables too where buffers move; both are rebuilt
+ *   on use.  mrq_device_ptr pointers and mrq_group_stride may change; the stride stays round_up(G, 128), at least 128.
+ * - Cost: a resize within the current stride allocates nothing; otherwise every new buffer is allocated before any old
+ *   one is freed and the surviving rows are copied on the device.  One kernel launch for a grow, none for a shrink.
+ * - Errors change nothing: n_groups >= 2^32 is MRQ_E_INVAL; a communicator or CUDA-IPC gather (mrq_comm_init,
+ *   mrq_ipc_prepare / mrq_ipc_attach) is MRQ_E_STATE, since every rank must own the same G; an allocation failure is
+ *   MRQ_E_NOMEM.  n_groups == G is a no-op.  */
+int mrq_resize_groups(mrq_engine *e, uint64_t n_groups);
+
 /* ---- the inbox: what node.Step(m) receives (reference raft.go:268-270) ---------------- */
 /* Dense form: one slot per (sender replica r, group g) per tick, replica-major [r*G + g].
  * Field meaning per type (raftpb.Message fields):

@@ -119,6 +119,7 @@ SIGNATURES = {
     "mrq_export_next": (C.c_int, [_EP, u64p]),
     "mrq_tick_count": (C.c_uint64, [_EP]),
     "mrq_set_tick_count": (C.c_int, [_EP, C.c_uint64]),
+    "mrq_resize_groups": (C.c_int, [_EP, C.c_uint64]),
     "mrq_post_inbox_dense": (C.c_int, [_EP, C.c_uint32, C.POINTER(Inbox)]),
     "mrq_post_inbox_delta": (C.c_int, [_EP, C.c_uint32, C.POINTER(Msg), C.c_size_t, C.c_int]),
     "mrq_post_inbox_packed": (C.c_int, [_EP, C.c_uint32, C.POINTER(InboxPacked)]),

@@ -144,6 +144,8 @@ struct mrq_engine {
   mrq_change *changes = nullptr;
   unsigned long long *change_count = nullptr;
   uint64_t change_cap = 0;
+  std::vector<bool> slot_out_live;  // per inbox slot: out_slot / delta_slot hold a tick of the current group count
+  bool gather_shared = false;       // mrq_comm_init / mrq_ipc_prepare sized the gather buffer for the peers
   std::string err;
 };
 
@@ -286,6 +288,17 @@ int ensure_compact(mrq_engine *e) {
   return MRQ_OK;
 }
 
+// Rows [g0, G) become fresh groups (init_state_kernel): one launch, whatever their number.
+int init_fresh_groups(mrq_engine *e, uint64_t g0) {
+  if (g0 >= e->G) return MRQ_OK;
+  const FreshRows f{e->commit_prev, e->pk_base_index, e->pk_base_term, e->c, e->compact_live ? 1 : 0};
+  init_state_kernel<<<nblocks(e->G - g0), 256, 0, e->stream>>>(e->s, f, g0, e->G, e->gs, e->cfg.group_base, e->R, e->cfg.self_id,
+                                                               e->cfg.seed, e->cfg.election_tick, e->cfg.heartbeat_tick, e->tick_no);
+  CK(e, cudaGetLastError());
+  e->launches++;
+  return MRQ_OK;
+}
+
 void fill_tick_args(mrq_engine *e, TickArgs &a) {
   a.s = e->s;
   a.ctr = e->ctr;
@@ -402,9 +415,11 @@ int launch_tick4(mrq_engine *e, const uint32_t *slots, uint32_t n) {
   e->slow_parity ^= 1u;
   if (A.t.world > 1) e->gather_prime = false;
   e->tick_no += n;
+  if (n > 1 && e->slot_out_live.size() < e->inbox.size()) e->slot_out_live.resize(e->inbox.size(), false);
   for (uint32_t k = 0; k < n; ++k) {
     PackedStage &sg = e->pk_stage[slots[k]];
     if (!sg.keep8) sg.frame8 = false;
+    if (n > 1) e->slot_out_live[slots[k]] = true;
     CK(e, cudaEventRecord(sg.consumed, e->stream));  // only now may the next frame overwrite the staging buffer
   }
   return MRQ_OK;
@@ -652,12 +667,7 @@ int mrq_create(const mrq_config *cfg, mrq_engine **out) {
       if ((r = dalloc(e, &ib.commit, gs * e->R))) return r;
       if ((r = dalloc(e, &ib.prop, gs))) return r;
     }
-    if (e->G) {
-      init_state_kernel<<<nblocks(e->G), 256, 0, e->stream>>>(e->s, e->G, cfg->group_base, e->R, cfg->self_id, cfg->seed,
-                                                             cfg->election_tick);
-      CK(e, cudaGetLastError());
-      e->launches++;
-    }
+    if ((r = init_fresh_groups(e, 0))) return r;
     CK(e, cudaStreamSynchronize(e->stream));
     return MRQ_OK;
   };
@@ -755,6 +765,139 @@ void *mrq_device_ptr(mrq_engine *e, int which) {
 }
 
 uint64_t mrq_group_stride(const mrq_engine *e) { return e ? e->gs : 0; }
+
+}  // extern "C"
+
+namespace {
+// A device buffer sized by the group stride: `rows` rows of gs elements of `elem` bytes.  `keep`: the rows of the groups
+// that survive a resize are copied into its replacement; every other buffer starts over zeroed, as mrq_create leaves it.
+struct StrideBuf {
+  void **at;
+  size_t elem, rows;
+  bool keep;
+};
+template <typename T>
+StrideBuf stride_buf(T *&p, size_t rows, bool keep) {
+  return StrideBuf{reinterpret_cast<void **>(&p), sizeof(T), rows, keep};
+}
+
+// Every buffer of the engine whose size follows the stride (scratch and staging are sized per call and follow alone).
+std::vector<StrideBuf> stride_bufs(mrq_engine *e) {
+  const size_t R = e->R;
+  std::vector<StrideBuf> v = {
+      stride_buf(e->s.term, 1, true),        stride_buf(e->s.meta, 1, true),          stride_buf(e->s.last_index, 1, true),
+      stride_buf(e->s.last_term, 1, true),   stride_buf(e->s.committed, 1, true),     stride_buf(e->s.term_start, 1, true),
+      stride_buf(e->s.match, R, true),       stride_buf(e->commit_prev, 1, true),     stride_buf(e->pk_base_index, 1, true),
+      stride_buf(e->pk_base_term, 1, true),  stride_buf(e->s.out, 1, false),          stride_buf(e->delta, 1, false),
+      stride_buf(e->gathered, 1, false),     stride_buf(e->slow_list, 1, false)};
+  if (e->compact_alloc) {
+    for (StrideBuf b : {stride_buf(e->c.flag, 1, true), stride_buf(e->c.commit, 1, true), stride_buf(e->c.win, 1, true),
+                        stride_buf(e->c.gate, 1, true), stride_buf(e->c.iblo, 1, true), stride_buf(e->c.match, R, true),
+                        stride_buf(e->c.ibase, 1, true), stride_buf(e->c.clk, 1, true), stride_buf(e->slow_list64, 1, false)})
+      v.push_back(b);
+  }
+  for (auto &ib : e->inbox)
+    for (StrideBuf b : {stride_buf(ib.type, R, false), stride_buf(ib.term, R, false), stride_buf(ib.index, R, false),
+                        stride_buf(ib.logterm, R, false), stride_buf(ib.commit, R, false), stride_buf(ib.prop, 1, false)})
+      v.push_back(b);
+  for (auto &p : e->out_slot)
+    if (p) v.push_back(stride_buf(p, 1, false));
+  for (auto &p : e->delta_slot)
+    if (p) v.push_back(stride_buf(p, 1, false));
+  return v;
+}
+
+// Move every stride-sized buffer to stride `gs`, keeping the rows of the first `keep` groups.  All new buffers are
+// allocated before any old one is freed, and the copies run on the device: a failure frees the new buffers only and
+// leaves the engine as it was.
+int restride(mrq_engine *e, uint64_t gs, uint64_t keep) {
+  const std::vector<StrideBuf> bufs = stride_bufs(e);
+  std::vector<void *> fresh(bufs.size(), nullptr);
+  auto drop_fresh = [&]() {
+    cudaStreamSynchronize(e->stream);
+    for (void *p : fresh)
+      if (p) cudaFree(p);
+  };
+  for (size_t k = 0; k < bufs.size(); ++k) {
+    const size_t bytes = bufs[k].elem * bufs[k].rows * gs;
+    if (cudaMalloc(&fresh[k], bytes) != cudaSuccess) {
+      cudaGetLastError();
+      fresh[k] = nullptr;
+      drop_fresh();
+      return fail(e, MRQ_E_NOMEM, "mrq_resize_groups: cannot allocate %zu bytes of device memory (the engine is unchanged)", bytes);
+    }
+  }
+  for (size_t k = 0; k < bufs.size(); ++k) {
+    const StrideBuf &b = bufs[k];
+    cudaError_t st = cudaMemsetAsync(fresh[k], 0, b.elem * b.rows * gs, e->stream);
+    if (st == cudaSuccess && b.keep && keep)
+      st = cudaMemcpy2DAsync(fresh[k], gs * b.elem, *b.at, e->gs * b.elem, keep * b.elem, b.rows, cudaMemcpyDeviceToDevice, e->stream);
+    if (st != cudaSuccess) {
+      drop_fresh();
+      return fail(e, MRQ_E_CUDA, "mrq_resize_groups: device copy failed: %s", cudaGetErrorString(st));
+    }
+  }
+  const cudaError_t st = cudaStreamSynchronize(e->stream);
+  if (st != cudaSuccess) {
+    drop_fresh();
+    return fail(e, MRQ_E_CUDA, "mrq_resize_groups: device copy failed: %s", cudaGetErrorString(st));
+  }
+  for (size_t k = 0; k < bufs.size(); ++k) {
+    cudaFree(*bufs[k].at);
+    *bufs[k].at = fresh[k];
+  }
+  e->gs = gs;
+  // mode-4 descriptor tables hold output pointers, and staging buffers are laid out by the stride
+  for (auto &kv : e->desc_tables) cudaFree(kv.second);
+  e->desc_tables.clear();
+  e->stage_gen++;
+  return MRQ_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int mrq_resize_groups(mrq_engine *e, uint64_t n_groups) {
+  if (!e) return MRQ_E_INVAL;
+  if (n_groups >= (1ull << 32)) return fail(e, MRQ_E_INVAL, "n_groups must be below 2^32 per engine (shard across engines)");
+  if (e->comm || e->ipc_attached || e->gather_shared)
+    return fail(e, MRQ_E_STATE, "mrq_resize_groups: the gather is shared with peers that own the same G (resize every rank's engine "
+                                "by recreating it)");
+  if (n_groups == e->G) return MRQ_OK;
+  CK(e, cudaSetDevice(e->device));
+  if (e->copy_stream) CK(e, cudaStreamSynchronize(e->copy_stream));  // a packed-inbox copy may still be filling a staging buffer
+  CK(e, cudaStreamSynchronize(e->stream));
+  const uint64_t old = e->G, keep = old < n_groups ? old : n_groups;
+  uint64_t gs = ((n_groups + 127) / 128) * 128;  // as mrq_create: a multiple of the tick CTA size, at least one CTA
+  if (gs == 0) gs = 128;
+  int r;
+  if (gs != e->gs) {
+    if ((r = restride(e, gs, keep))) return r;
+  } else {  // the buffers stay: clear what mrq_create leaves zeroed and the groups do not own
+    CK(e, cudaMemsetAsync(e->s.out, 0, e->gs * sizeof(uint32_t), e->stream));
+    CK(e, cudaMemsetAsync(e->delta, 0, e->gs, e->stream));
+    for (auto &ib : e->inbox) {  // (mrq_clear_inbox)
+      CK(e, cudaMemsetAsync(ib.type, 0, e->gs * e->R, e->stream));
+      CK(e, cudaMemsetAsync(ib.prop, 0, e->gs * sizeof(uint32_t), e->stream));
+    }
+  }
+  // Captured graphs hold G and the buffer addresses by value.  Waiting frames and the outputs of earlier ticks describe
+  // the old group count: every slot starts over empty, as after mrq_create.
+  for (auto &kv : e->graphs) cudaGraphExecDestroy(kv.second);
+  e->graphs.clear();
+  for (auto &sg : e->pk_stage) sg.frame8 = sg.keep8 = false;
+  e->slot_out_live.assign(e->slot_out_live.size(), false);
+  e->last_out = nullptr;
+  e->last_delta = nullptr;
+  e->G = n_groups;
+  e->cfg.n_groups = n_groups;
+  // While G == 0 no kernel runs to advance the device's tick number (TickArgs::tick_cur): bring it to the host's count,
+  // which keys the groups' timeout draws from their first tick on.
+  CK(e, cudaMemcpyAsync(e->tickbuf + (e->tick_parity & 1u), &e->tick_no, sizeof e->tick_no, cudaMemcpyHostToDevice, e->stream));
+  if ((r = init_fresh_groups(e, old))) return r;
+  CK(e, cudaStreamSynchronize(e->stream));
+  return MRQ_OK;
+}
 
 void *mrq_alloc_pinned(size_t bytes) {
   void *p = nullptr;
@@ -1713,7 +1856,8 @@ int mrq_drain_tick_deltas(mrq_engine *e, uint8_t *delta_out_pinned) {
 int mrq_sync_slot_outputs(mrq_engine *e, uint32_t slot, uint32_t *out_words, uint8_t *delta_out) {
   int r = check_slot(e, slot);
   if (r) return r;
-  if (slot >= e->out_slot.size() || !e->out_slot[slot] || !e->delta_slot[slot])
+  if (slot >= e->out_slot.size() || !e->out_slot[slot] || !e->delta_slot[slot] || slot >= e->slot_out_live.size() ||
+      !e->slot_out_live[slot])
     return fail(e, MRQ_E_STATE, "slot %u was not part of a mode-4 mrq_tick_many sequence", slot);
   CK(e, cudaSetDevice(e->device));
   if (e->G && out_words) CK(e, cudaMemcpyAsync(out_words, e->out_slot[slot], e->G * 4, cudaMemcpyDeviceToHost, e->stream));
@@ -1861,6 +2005,7 @@ int mrq_comm_init(mrq_engine *e, const uint8_t id[MRQ_COMM_ID_BYTES], uint32_t r
   memcpy(&uid, id, MRQ_COMM_ID_BYTES);
   int st = g_nccl.CommInitRank(&e->comm, (int)world, uid, (int)rank);
   if (st != 0) return fail(e, MRQ_E_NCCL, "ncclCommInitRank failed: %s", g_nccl.GetErrorString ? g_nccl.GetErrorString(st) : "?");
+  e->gather_shared = true;
   e->world = world;
   e->rank = rank;
   return MRQ_OK;
@@ -1887,7 +2032,10 @@ int mrq_ipc_export(mrq_engine *e, uint8_t handle_out[MRQ_IPC_HANDLE_BYTES]) {
 int mrq_ipc_prepare(mrq_engine *e, uint32_t world) {
   if (!e || world < 1 || world > 8) return MRQ_E_INVAL;
   CK(e, cudaSetDevice(e->device));
-  return ensure_gather(e, world);
+  int r = ensure_gather(e, world);
+  if (r) return r;
+  e->gather_shared = true;  // the buffer's handle may be exported from here on
+  return MRQ_OK;
 }
 
 int mrq_ipc_attach(mrq_engine *e, const uint8_t *handles, uint32_t rank, uint32_t world) {

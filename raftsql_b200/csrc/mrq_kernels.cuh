@@ -2881,17 +2881,48 @@ __global__ void fix_strict_kernel(StateView s, uint64_t G, uint64_t gs, uint32_t
   s.meta[i] = meta_pack(m);
 }
 
-__global__ void init_state_kernel(StateView s, uint64_t G, uint64_t group_base, uint32_t R, uint32_t self_id, uint64_t seed,
-                                  uint32_t election_tick) {
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= G) return;
+// Where a fresh group's rows live besides the wide columns: the commit-delta drain base, the packed-inbox decode bases,
+// and, while tick mode 4's compact state is live (`compact`), the compact columns.
+struct FreshRows {
+  uint64_t *commit_prev, *base_index, *base_term;
+  CompactViewT<CompactOff> c;
+  int compact;
+};
+
+// A fresh group: what mrq_create makes of every group and mrq_resize_groups of every group a grow adds.  newRaft() on
+// empty storage: a follower at term 0 with an empty log in every wide column of row i, its drain base and packed bases
+// 0, and, with the compact state live, its compact form at `T` (the number of the next tick to run), so that a grow
+// leaves the next mode-4 tick nothing to re-compact.  Every column of the row is written: after a shrink within the
+// stride the row still holds a dropped group.
+template <typename Off>
+__device__ __forceinline__ void init_group(const StateView &s, uint64_t *commit_prev, uint64_t *base_index, uint64_t *base_term,
+                                           const CompactViewT<Off> &c, const bool compact, uint64_t gs, uint32_t R, const uint64_t i,
+                                           uint64_t group_base, uint32_t self_id, uint64_t seed, uint32_t et, uint32_t ht, uint64_t T) {
   Meta m{};
   m.role = MRQ_ROLE_FOLLOWER;
   m.self = self_id ? self_id : (uint32_t)((group_base + i) % R) + 1u;
-  m.rto = mrq_randomized_timeout(seed, group_base + i, 0, election_tick);  // newRaft(): becomeFollower -> reset()
+  m.rto = mrq_randomized_timeout(seed, group_base + i, 0, et);  // newRaft(): becomeFollower -> reset()
   m.ltok = 1;  // term 0, empty log: lastTerm() == Term
+  s.term[i] = 0;
   s.meta[i] = meta_pack(m);
+  s.last_index[i] = 0;
+  s.last_term[i] = 0;
+  s.committed[i] = 0;
   s.term_start[i] = kNoGate;
+  for (uint32_t r = 0; r < R; ++r) s.match[(uint64_t)r * gs + i] = 0;
+  commit_prev[i] = 0;
+  base_index[i] = 0;
+  base_term[i] = 0;
+  if (compact) compact_group(s, c, base_index, base_term, gs, R, i, T, et, ht);
+}
+
+// Rows [g0, G) become fresh groups (g0 = 0: mrq_create; g0 = the old G: a grow).
+__global__ void init_state_kernel(StateView s, FreshRows f, uint64_t g0, uint64_t G, uint64_t gs, uint64_t group_base, uint32_t R,
+                                  uint32_t self_id, uint64_t seed, uint32_t election_tick, uint32_t heartbeat_tick, uint64_t T) {
+  const uint64_t i = g0 + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= G) return;
+  init_group(s, f.commit_prev, f.base_index, f.base_term, f.c, f.compact != 0, gs, R, i, group_base, self_id, seed, election_tick,
+             heartbeat_tick, T);
 }
 
 __global__ void export_next_kernel(const uint64_t *match, const uint64_t *term_start, uint64_t *next, uint64_t G, uint64_t gs,

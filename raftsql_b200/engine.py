@@ -170,6 +170,13 @@ class Engine:
     def tick_count(self, t: int):
         self._ck(self.L.mrq_set_tick_count(self.h, t))
 
+    def resize_groups(self, n: int):
+        """Hold n groups: fresh groups are added at the tail, or the last ones dropped; the others keep their state.
+        Every inbox slot is cleared, and arrays this wrapper returns from now on have n groups."""
+        self._ck(self.L.mrq_resize_groups(self.h, n))
+        self.G = int(n)
+        self.cfg.n_groups = self.G
+
     # -- inbox -----------------------------------------------------------------------------
     def post_inbox_dense(self, ib: dict, slot: int = 0):
         v = F.Inbox()
